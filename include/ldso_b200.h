@@ -201,6 +201,25 @@ int ldso_b200_optimize_begin(ldso_b200_ctx *ctx, double *energy_out);
  * first_iteration.. are passed to solveSystemF (orthogonalize from iteration 2). Asynchronous on the
  * context's stream; results are fetched with the getters below (which synchronise). */
 int ldso_b200_gn_iterations(ldso_b200_ctx *ctx, int first_iteration, int n_iterations);
+/* FullSystem::optimize's loop with its exit (FullSystem.cc:777-831): at most max_iterations bodies (as gn_iterations runs them)
+ * numbered from first_iteration; the loop stops after the body whose doStepFromBackup returned canbreak once that body's
+ * iteration >= min_iterations (`if (canbreak && iteration >= setting_minOptIterations) break;`, :829; setting_minOptIterations
+ * = 1, Setting.cc:37). max_iterations == 0 launches nothing. Asynchronous like gn_iterations: the decision is taken on the
+ * device, inside one CUDA graph with a conditional WHILE node. Where the driver cannot build that node, without CUDA graphs
+ * (LDSO_B200_NO_GRAPH) and while kernel_times is collecting, the same kernels run host-driven with one synchronise per body.
+ * Either way the results are the same bits. With the peer exchange every rank takes the same decision after the same body. */
+int ldso_b200_gn_iterations_until(ldso_b200_ctx *ctx, int first_iteration, int max_iterations, int min_iterations);
+/* number of bodies the last gn_iterations_until (or optimize_from_host_until*) ran; synchronises */
+int ldso_b200_get_iterations_run(ldso_b200_ctx *ctx, int *n);
+/* which form the last gn_iterations_until ran in */
+#define LDSO_B200_UNTIL_HOST 0          /* host-driven, one synchronise per body */
+#define LDSO_B200_UNTIL_GRAPH_PDL 1     /* conditional WHILE node, programmatic dependent launch between the body's kernels */
+#define LDSO_B200_UNTIL_GRAPH 2         /* conditional WHILE node, full dependencies between the body's kernels */
+int ldso_b200_get_until_form(ldso_b200_ctx *ctx, int *form);
+/* FullSystem::optimize's iteration budget (FullSystem.cc:727-732): 0 for nFrames < 2, 15 for nFrames < 4 (the `< 3 -> 20`
+ * assignment is overwritten by the `< 4 -> 15` one), else max_opt_iterations (setting_maxOptIterations = 6, Setting.cc:36).
+ * Needs no context; returns the budget, or LDSO_B200_ERR_ARG for a negative max_opt_iterations. */
+int ldso_b200_optimize_iteration_budget(int nFrames, int max_opt_iterations);
 /* ---- one call per keyframe optimisation, from host buffers ------------------------------------------------
  * What FullSystem::optimize does around the loop, as ONE call: (optionally) the newest keyframe's raw image -> device
  * makeImages, set_frames, set_window, the optimize() prologue, n_iterations Gauss-Newton iterations, and the read-back of the
@@ -229,6 +248,13 @@ int ldso_b200_optimize_from_host(ldso_b200_ctx *ctx, const ldso_b200_fused_io *i
  * uploads of one window then overlap the kernels of the other (FullSystem keeps mapping and tracking on separate threads the same way). */
 int ldso_b200_optimize_from_host_submit(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io);
 int ldso_b200_optimize_from_host_wait(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io);
+/* The same three calls with FullSystem::optimize's exit: the loop is gn_iterations_until(io->first_iteration, io->n_iterations,
+ * min_iterations), so io->n_iterations is the MAXIMUM (pass ldso_b200_optimize_iteration_budget(nFrames, setting_maxOptIterations)).
+ * *iterations_run (may be NULL) receives the number of bodies run; it rides back with the other results, so _until_submit /
+ * _until_wait keep the two-context overlap of the pair above. */
+int ldso_b200_optimize_from_host_until(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, int min_iterations, int *iterations_run);
+int ldso_b200_optimize_from_host_until_submit(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, int min_iterations);
+int ldso_b200_optimize_from_host_until_wait(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, int *iterations_run);
 
 /* Multi-GPU (SURVEY §8e): points are sharded over ranks (one context per GPU), frames/images replicated. A GN
  * iteration is split around the ONE collective: gn_phase_a(iteration) runs [solve + frame step of `iteration`

@@ -69,7 +69,9 @@ SYMBOLS = [
     "ldso_b200_download_frame_level", "ldso_b200_set_window", "ldso_b200_set_frames", "ldso_b200_set_marg_prior",
     "ldso_b200_get_marg_prior", "ldso_b200_linearize_all", "ldso_b200_apply_res", "ldso_b200_backup_state",
     "ldso_b200_solve_system", "ldso_b200_get_system", "ldso_b200_do_step", "ldso_b200_marginalize_points", "ldso_b200_marginalize_frame", "ldso_b200_calc_energies", "ldso_b200_accumulate", "ldso_b200_select_activation", "ldso_b200_init_calc_res", "ldso_b200_optimize_begin",
-    "ldso_b200_gn_iterations", "ldso_b200_optimize_from_host", "ldso_b200_optimize_from_host_submit", "ldso_b200_optimize_from_host_wait", "ldso_b200_reduce_buffer", "ldso_b200_set_shard", "ldso_b200_gn_phase_a",
+    "ldso_b200_gn_iterations", "ldso_b200_gn_iterations_until", "ldso_b200_get_iterations_run", "ldso_b200_get_until_form",
+    "ldso_b200_optimize_iteration_budget", "ldso_b200_optimize_from_host_until", "ldso_b200_optimize_from_host_until_submit",
+    "ldso_b200_optimize_from_host_until_wait", "ldso_b200_optimize_from_host", "ldso_b200_optimize_from_host_submit", "ldso_b200_optimize_from_host_wait", "ldso_b200_reduce_buffer", "ldso_b200_set_shard", "ldso_b200_gn_phase_a",
     "ldso_b200_gn_phase_b", "ldso_b200_peer_export", "ldso_b200_peer_connect", "ldso_b200_peer_error", "ldso_b200_prefetch_results", "ldso_b200_get_energy", "ldso_b200_get_last_solution", "ldso_b200_get_points",
     "ldso_b200_get_residuals", "ldso_b200_get_frames", "ldso_b200_get_nullspace_projector", "ldso_b200_immature_init",
     "ldso_b200_trace_immature", "ldso_b200_optimize_immature", "ldso_b200_tracker_make_k",
@@ -103,6 +105,18 @@ def load():
                 fn.restype = C.c_int
         _lib = L
     return _lib
+
+
+UNTIL_FORMS = {0: "host", 1: "graph+pdl", 2: "graph"}     # LDSO_B200_UNTIL_*
+
+
+def optimize_iteration_budget(nF, max_its=6) -> int:
+    """FullSystem::optimize's iteration budget for a window of nF keyframes (0 below 2, 15 below 4, else max_its =
+    setting_maxOptIterations)."""
+    r = load().ldso_b200_optimize_iteration_budget(int(nF), int(max_its))
+    if r < 0:
+        raise Error(f"ldso_b200_optimize_iteration_budget({nF}, {max_its}) failed: {r}")
+    return r
 
 
 def default_settings() -> Settings:
@@ -327,6 +341,22 @@ class Context:
 
     def gn_iterations(self, first, n):
         self._chk(self.L.ldso_b200_gn_iterations(self.ctx, int(first), int(n)))
+
+    def gn_iterations_until(self, first, max_its, min_its=1):
+        """At most max_its bodies from iteration `first`, stopping after the body whose canbreak fired at iteration >= min_its
+        (FullSystem::optimize's exit). Asynchronous; iterations_run() gives the count."""
+        self._chk(self.L.ldso_b200_gn_iterations_until(self.ctx, int(first), int(max_its), int(min_its)))
+
+    def iterations_run(self) -> int:
+        n = C.c_int()
+        self._chk(self.L.ldso_b200_get_iterations_run(self.ctx, C.byref(n)))
+        return n.value
+
+    def until_form(self) -> str:
+        """'graph+pdl', 'graph' (conditional WHILE node) or 'host' (host-driven): the form of the last gn_iterations_until."""
+        f = C.c_int()
+        self._chk(self.L.ldso_b200_get_until_form(self.ctx, C.byref(f)))
+        return UNTIL_FORMS[f.value]
 
     def reduce_buffer(self):
         p = C.c_void_p()
@@ -647,6 +677,32 @@ class StepIO:
         self.ctx._chk(self.L.ldso_b200_optimize_from_host(self.h, C.byref(self._io)))
         self.ctx.nF, self.ctx.nP, self.ctx.nR = self.nF, self.nP, self.nR
         return self.out
+
+    def submit_until(self, iteration=0, max_iterations=6, min_iterations=1):
+        """ldso_b200_optimize_from_host_until_submit: the step with FullSystem::optimize's exit, not waited for."""
+        self._prep(iteration, max_iterations)
+        self.ctx._chk(self.L.ldso_b200_optimize_from_host_until_submit(self.h, C.byref(self._io), int(min_iterations)))
+
+    def wait_until(self):
+        """ldso_b200_optimize_from_host_until_wait: outputs filled, self.iterations_run = bodies run."""
+        n = C.c_int()
+        self.ctx._chk(self.L.ldso_b200_optimize_from_host_until_wait(self.h, C.byref(self._io), C.byref(n)))
+        self.ctx.nF, self.ctx.nP, self.ctx.nR = self.nF, self.nP, self.nR
+        self.iterations_run = n.value
+        return self.out
+
+    def fused_until(self, iteration=0, max_iterations=6, min_iterations=1):
+        """ldso_b200_optimize_from_host_until: the whole step with the exit as ONE call; self.iterations_run = bodies run."""
+        self._prep(iteration, max_iterations)
+        n = C.c_int()
+        self.ctx._chk(self.L.ldso_b200_optimize_from_host_until(self.h, C.byref(self._io), int(min_iterations), C.byref(n)))
+        self.ctx.nF, self.ctx.nP, self.ctx.nR = self.nF, self.nP, self.nR
+        self.iterations_run = n.value
+        return self.out
+
+    def scalars(self):
+        """(energy, canbreak) the last fused / submitted step returned"""
+        return float(self._scal[0][0]), bool(self._scal[1][0])
 
     def _prep(self, iteration, n_iterations):
         if not hasattr(self, "_io"):

@@ -19,6 +19,7 @@
 #include "tracker_kernels.cuh"
 #include "trace_types.h"
 #include "posegraph.cuh"
+#include "gn_loop.cuh"
 
 static_assert(K1_THREADS / 32 == MAXF, "phase B maps one warp to one target frame");
 
@@ -81,6 +82,15 @@ struct ldso_b200_ctx {
     // one GN iteration (K3 -> K1 -> K2a -> K2b) captured as a CUDA graph; re-captured when the window arena changes
     cudaGraphExec_t gn_graph = nullptr;
     bool gn_graph_valid = false;
+    // the same body closed by k_gn_continue inside a conditional WHILE node (gn_iterations_until); same validity as gn_graph
+    cudaGraphExec_t until_graph = nullptr;
+    bool until_graph_valid = false;
+    int until_form = LDSO_B200_UNTIL_HOST;    // which form the last gn_iterations_until ran (ldso_b200_get_until_form)
+    int until_graph_form = LDSO_B200_UNTIL_GRAPH;     // ... and which one until_graph holds
+    bool until_cond = true;          // cleared for good when the driver refuses the conditional node
+    int until_launches_per_body = 0; // kernels per body of the last WHILE-node launch, not yet in `launches`
+    int *loop_dev = nullptr;         // k_gn_continue's parameters and counters (LOOP_*)
+    int *loop_pin = nullptr;         // pinned: the host-driven form reads LOOP_CONT back here
     bool use_graph = true;
     bool use_pdl = true;             // programmatic dependent launch inside the GN iteration (env LDSO_B200_NO_PDL disables)
     bool pdl_now = false;            // set while launch_gn_body issues its four kernels
@@ -209,6 +219,8 @@ extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_lev
     ok = ok && cudaMalloc(&c->ws_dev, sizeof(WinState)) == cudaSuccess;
     ok = ok && cudaMallocHost(&c->ws_host, sizeof(WinState)) == cudaSuccess;
     ok = ok && cudaMalloc(&c->iteration_dev, sizeof(int)) == cudaSuccess;
+    ok = ok && cudaMalloc(&c->loop_dev, sizeof(int) * LOOP_WORDS) == cudaSuccess;
+    ok = ok && cudaMallocHost(&c->loop_pin, sizeof(int) * LOOP_WORDS) == cudaSuccess;
     // solve buffers: 4 + 1 + 1 + 1 matrices (n x n) and 6 vectors
     const size_t nn = (size_t) MAXN * MAXN;
     ok = ok && cudaMalloc(&c->solve_mem, sizeof(double) * (7 * nn + 8 * MAXN)) == cudaSuccess;
@@ -220,6 +232,7 @@ extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_lev
     cudaMemset(c->solve_mem, 0, sizeof(double) * (7 * nn + 8 * MAXN));
     cudaMemset(c->trk_counter, 0, sizeof(unsigned));
     cudaMemset(c->iteration_dev, 0, sizeof(int));
+    cudaMemset(c->loop_dev, 0, sizeof(int) * LOOP_WORDS);
     cudaMemset(c->ws_dev, 0, sizeof(WinState));
     memset(c->ws_host, 0, sizeof(WinState));
     double *p = c->solve_mem;
@@ -255,7 +268,7 @@ static void free_window(ldso_b200_ctx *c) {
     if (c->arena_dev) { cudaFree(c->arena_dev); c->arena_dev = nullptr; }
     if (c->arena_host) { cudaFreeHost(c->arena_host); c->arena_host = nullptr; }
     { c->mirror_valid = false; c->results_inflight = false; c->sol_valid = false; c->mirror_full_valid = false; }
-    c->gn_graph_valid = false;
+    c->gn_graph_valid = false; c->until_graph_valid = false;
     c->have_window = false;
 }
 
@@ -265,6 +278,7 @@ extern "C" void ldso_b200_destroy(ldso_b200_ctx *c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     c->kt_report();
     if (c->gn_graph) cudaGraphExecDestroy(c->gn_graph);
+    if (c->until_graph) cudaGraphExecDestroy(c->until_graph);
     free_window(c);
     for (int s = 0; s < NSLOTS; s++) for (int l = 0; l < MAXLVL; l++) if (c->img[s][l]) cudaFree(c->img[s][l]);
     for (int l = 0; l < MAXLVL; l++) for (int k = 0; k < 4; k++) if (c->trk_pc[l][k]) cudaFree(c->trk_pc[l][k]);
@@ -283,6 +297,8 @@ extern "C" void ldso_b200_destroy(ldso_b200_ctx *c) {
     if (c->peer_words) cudaFree(c->peer_words);
     if (c->red_sum) cudaFree(c->red_sum);
     if (c->iteration_dev) cudaFree(c->iteration_dev);
+    if (c->loop_dev) cudaFree(c->loop_dev);
+    if (c->loop_pin) cudaFreeHost(c->loop_pin);
     if (c->solve_mem) cudaFree(c->solve_mem);
     if (c->trk_partials) cudaFree(c->trk_partials);
     if (c->trk_counter) cudaFree(c->trk_counter);
@@ -588,7 +604,7 @@ static int build_derived(ldso_b200_ctx *c) {
         return c->fail(LDSO_B200_ERR_STATE, "the window's newest-frame residual count changed: the peer exchange buffers must be re-exported");
     d.items = items_dev; d.host_item_begin = hib_dev; d.res_newest_slot = slot_dev;
     c->derived_dirty = false;
-    c->gn_graph_valid = false;
+    c->gn_graph_valid = false; c->until_graph_valid = false;
     return LDSO_B200_OK;
 }
 
@@ -1434,6 +1450,136 @@ extern "C" int ldso_b200_gn_iterations(ldso_b200_ctx *c, int first_iteration, in
     return LDSO_B200_OK;
 }
 
+// ---- FullSystem::optimize's iteration budget and convergence exit (FullSystem.cc:727-732, :829)
+extern "C" int ldso_b200_optimize_iteration_budget(int nFrames, int max_opt_iterations) {
+    if (max_opt_iterations < 0) return LDSO_B200_ERR_ARG;
+    if (nFrames < 2) return 0;
+    if (nFrames < 4) return 15;          // the `< 3 -> 20` assignment (:729-730) is overwritten by `< 4 -> 15` (:731-732)
+    return max_opt_iterations;
+}
+
+static int launch_continue(ldso_b200_ctx *c, cudaGraphConditionalHandle cond, int use_cond) {
+    c->pdl_now = true;
+    launch_loop_kernel(c, k_gn_continue, dim3(1), dim3(32), 0, (const WinState *) c->ws_dev, (const int *) c->iteration_dev, c->loop_dev,
+                       cond, use_cond);
+    c->pdl_now = false;
+    LAUNCH_CHECK(c);
+    return LDSO_B200_OK;
+}
+
+// One graph holding a conditional WHILE node whose body is the captured GN body + k_gn_continue. The node's condition starts at 1
+// on every launch; the continue kernel clears it after the body that ends the loop. Where the driver refuses programmatic edges
+// inside the body the capture is repeated with full dependencies; where it refuses conditional nodes at all, until_cond is
+// cleared and gn_iterations_until runs its host-driven form from then on. Returns an error only for a launch the body itself
+// rejects (the same errors gn_iterations reports).
+static int capture_until_graph(ldso_b200_ctx *c) {
+    if (c->until_graph) { cudaGraphExecDestroy(c->until_graph); c->until_graph = nullptr; }
+    const bool pdl_saved = c->use_pdl;
+    int rc_last = 0;
+    for (int attempt = 0; attempt < 2; attempt++) {
+        if (attempt == 1) {
+            if (!pdl_saved) break;
+            c->use_pdl = false;
+        }
+        cudaGraph_t g = nullptr;
+        cudaGraphConditionalHandle cond = 0;
+        cudaGraphNode_t node = nullptr;
+        cudaGraphNodeParams p = {cudaGraphNodeTypeConditional};
+        int rc = 0;
+        cudaError_t e = cudaGraphCreate(&g, 0);
+        if (e == cudaSuccess) e = cudaGraphConditionalHandleCreate(&cond, g, 1, cudaGraphCondAssignDefault);
+        if (e == cudaSuccess) {
+            p.conditional.handle = cond;
+            p.conditional.type = cudaGraphCondTypeWhile;
+            p.conditional.size = 1;
+            e = cudaGraphAddNode(&node, g, nullptr, 0, &p);
+        }
+        if (e == cudaSuccess) e = cudaStreamBeginCaptureToGraph(c->stream, p.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal);
+        if (e == cudaSuccess) {
+            const long long l0 = c->launches;
+            rc = launch_gn_body(c);
+            if (!rc) rc = launch_continue(c, cond, 1);
+            cudaGraph_t body = nullptr;      // the node's own body graph, owned by g
+            const cudaError_t e2 = cudaStreamEndCapture(c->stream, &body);
+            c->launches = l0;
+            e = e2;
+        }
+        if (rc == 0 && e == cudaSuccess) {
+            e = cudaGraphInstantiate(&c->until_graph, g, 0);
+            if (e != cudaSuccess) c->until_graph = nullptr;
+        }
+        if (g) cudaGraphDestroy(g);
+        c->use_pdl = pdl_saved;
+        if (rc == 0 && e == cudaSuccess) {
+            c->until_graph_valid = true;
+            c->until_graph_form = (attempt == 0 && pdl_saved) ? LDSO_B200_UNTIL_GRAPH_PDL : LDSO_B200_UNTIL_GRAPH;
+            return LDSO_B200_OK;
+        }
+        cudaGetLastError();
+        rc_last = rc;
+    }
+    if (rc_last) return rc_last;
+    c->until_cond = false;
+    return LDSO_B200_OK;
+}
+
+// bodies a WHILE-node launch ran enter launch_count once their number is known on the host
+static void count_until_launches(ldso_b200_ctx *c, int bodies) {
+    c->launches += (long long) bodies * c->until_launches_per_body;
+    c->until_launches_per_body = 0;
+}
+
+extern "C" int ldso_b200_gn_iterations_until(ldso_b200_ctx *c, int first_iteration, int max_iterations, int min_iterations) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    if (max_iterations < 0) return c->fail(LDSO_B200_ERR_ARG, "negative iteration count");
+    if (c->multi && !c->peers_connected) return c->fail(LDSO_B200_ERR_STATE, "sharded context without peer exchange: use gn_phase_a / all-reduce / gn_phase_b, or peer_export + peer_connect");
+    cudaSetDevice(c->device);
+    RET_IF(build_derived(c));
+    RET_IF(ensure_solve_ready(c));
+    const int params[LOOP_CONT] = {max_iterations, min_iterations, 0};      // LOOP_MAX, LOOP_MIN, LOOP_RUN
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->loop_dev, params, sizeof(params), cudaMemcpyHostToDevice, c->stream));
+    c->until_launches_per_body = 0;
+    if (max_iterations == 0) return LDSO_B200_OK;
+    RET_IF(set_iteration(c, first_iteration));
+    if (c->use_graph && c->until_cond && c->d.nItems > 0) {
+        if (!c->until_graph_valid) RET_IF(capture_until_graph(c));
+        if (c->until_graph_valid) {
+            CUDA_CHECK_RET(c, cudaGraphLaunch(c->until_graph, c->stream));
+            c->until_form = c->until_graph_form;
+            c->until_launches_per_body = c->peers_connected ? 6 : 5;
+            c->select_pending = true;
+            { c->mirror_valid = false; c->results_inflight = false; c->sol_valid = false; c->mirror_full_valid = false; }
+            return LDSO_B200_OK;
+        }
+    }
+    // host-driven: the same kernels, one synchronise per body to read the continue kernel's decision
+    c->until_form = LDSO_B200_UNTIL_HOST;
+    for (int i = 0; i < max_iterations; i++) {
+        RET_IF(launch_gn_body(c));
+        RET_IF(launch_continue(c, 0, 0));
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(c->loop_pin, c->loop_dev + LOOP_CONT, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+        if (!*c->loop_pin) break;
+    }
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_get_iterations_run(ldso_b200_ctx *c, int *n) {
+    if (!c || !n) return LDSO_B200_ERR_ARG;
+    cudaSetDevice(c->device);
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->loop_pin + LOOP_RUN, c->loop_dev + LOOP_RUN, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    *n = c->loop_pin[LOOP_RUN];
+    count_until_launches(c, *n);
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_get_until_form(ldso_b200_ctx *c, int *form) {
+    if (!c || !form) return LDSO_B200_ERR_ARG;
+    *form = c->until_form;
+    return LDSO_B200_OK;
+}
+
 static int wait_results(ldso_b200_ctx *c);
 extern "C" int ldso_b200_prefetch_results(ldso_b200_ctx *c);
 extern "C" int ldso_b200_get_points(ldso_b200_ctx *c, float *idepth, float *idepth_zero, float *step, float *HdiF, float *bdSumF, float *Hdd,
@@ -1445,7 +1591,9 @@ extern "C" int ldso_b200_get_residuals(ldso_b200_ctx *c, uint8_t *state_state, u
 // stream and return WITHOUT waiting. The caller's buffers (io->image, frames, window arrays) are consumed before this returns except
 // io->image, which must stay valid until the matching _wait. Two contexts fed alternately overlap one window's uploads with the
 // other's kernels (bench.py's pipelined end-to-end leg); a single context just splits the call at its only synchronisation point.
-extern "C" int ldso_b200_optimize_from_host_submit(ldso_b200_ctx *c, const ldso_b200_fused_io *io) {
+// until: the loop runs with FullSystem::optimize's exit (gn_iterations_until, io->n_iterations the maximum) and the number of bodies
+// it ran rides into pinned staging behind the other two scalars
+static int submit_impl(ldso_b200_ctx *c, const ldso_b200_fused_io *io, bool until, int min_iterations) {
     if (!c || !io || !io->frames || !io->window || !io->calib_value_scaled || !io->calib_value_zero) return LDSO_B200_ERR_ARG;
     if (io->n_iterations < 0) return c->fail(LDSO_B200_ERR_ARG, "negative iteration count");
     // the image first: 1.2 MB over PCIe, in flight while the host packs the frame states and the window
@@ -1453,14 +1601,18 @@ extern "C" int ldso_b200_optimize_from_host_submit(ldso_b200_ctx *c, const ldso_
     RET_IF(ldso_b200_set_frames(c, io->nFrames, io->frames, io->calib_value_scaled, io->calib_value_zero));
     RET_IF(ldso_b200_set_window(c, io->window));
     RET_IF(ldso_b200_optimize_begin(c, nullptr));
-    if (io->n_iterations > 0) RET_IF(ldso_b200_gn_iterations(c, io->first_iteration, io->n_iterations));
+    if (until) RET_IF(ldso_b200_gn_iterations_until(c, io->first_iteration, io->n_iterations, min_iterations));
+    else if (io->n_iterations > 0) RET_IF(ldso_b200_gn_iterations(c, io->first_iteration, io->n_iterations));
     RET_IF(ldso_b200_prefetch_results(c));
-    // the two scalars ride behind the prefetch into pinned staging (sol_host has MAXN spare doubles behind lastX)
+    // the scalars ride behind the prefetch into pinned staging (sol_host has MAXN spare doubles behind lastX)
     const size_t nn = (size_t) MAXN * MAXN;
     CUDA_CHECK_RET(c, cudaMemcpyAsync(c->sol_host + nn + 2 * MAXN, &c->ws_dev->energy, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaMemcpyAsync(c->sol_host + nn + 2 * MAXN + 1, &c->ws_dev->canbreak, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    if (until) CUDA_CHECK_RET(c, cudaMemcpyAsync(c->sol_host + nn + 2 * MAXN + 2, c->loop_dev + LOOP_RUN, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     return LDSO_B200_OK;
 }
+
+extern "C" int ldso_b200_optimize_from_host_submit(ldso_b200_ctx *c, const ldso_b200_fused_io *io) { return submit_impl(c, io, false, 0); }
 
 extern "C" int ldso_b200_optimize_from_host_wait(ldso_b200_ctx *c, const ldso_b200_fused_io *io) {
     if (!c || !io) return LDSO_B200_ERR_ARG;
@@ -1480,6 +1632,24 @@ extern "C" int ldso_b200_optimize_from_host_wait(ldso_b200_ctx *c, const ldso_b2
 extern "C" int ldso_b200_optimize_from_host(ldso_b200_ctx *c, const ldso_b200_fused_io *io) {
     RET_IF(ldso_b200_optimize_from_host_submit(c, io));
     return ldso_b200_optimize_from_host_wait(c, io);
+}
+
+extern "C" int ldso_b200_optimize_from_host_until_submit(ldso_b200_ctx *c, const ldso_b200_fused_io *io, int min_iterations) {
+    return submit_impl(c, io, true, min_iterations);
+}
+
+extern "C" int ldso_b200_optimize_from_host_until_wait(ldso_b200_ctx *c, const ldso_b200_fused_io *io, int *iterations_run) {
+    RET_IF(ldso_b200_optimize_from_host_wait(c, io));
+    int n = 0;
+    memcpy(&n, c->sol_host + (size_t) MAXN * MAXN + 2 * MAXN + 2, sizeof(int));
+    count_until_launches(c, n);
+    if (iterations_run) *iterations_run = n;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_optimize_from_host_until(ldso_b200_ctx *c, const ldso_b200_fused_io *io, int min_iterations, int *iterations_run) {
+    RET_IF(ldso_b200_optimize_from_host_until_submit(c, io, min_iterations));
+    return ldso_b200_optimize_from_host_until_wait(c, io, iterations_run);
 }
 
 extern "C" int ldso_b200_reduce_buffer(ldso_b200_ctx *c, void **buf_dev, size_t *n_doubles) {
@@ -1552,7 +1722,7 @@ extern "C" int ldso_b200_peer_connect(ldso_b200_ctx *c, int rank, int world, con
     c->px.epoch = c->peer_words; c->px.done = (unsigned *) (c->peer_words + 1); c->px.error = c->peer_words + 2;
     c->px.out = c->red_sum;
     c->peers_connected = true;
-    c->gn_graph_valid = false;
+    c->gn_graph_valid = false; c->until_graph_valid = false;
     return LDSO_B200_OK;
 }
 
