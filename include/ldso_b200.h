@@ -256,6 +256,42 @@ int ldso_b200_optimize_from_host_until(ldso_b200_ctx *ctx, const ldso_b200_fused
 int ldso_b200_optimize_from_host_until_submit(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, int min_iterations);
 int ldso_b200_optimize_from_host_until_wait(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, int *iterations_run);
 
+/* ---- the end of FullSystem::optimize (FullSystem.cc:833-863), after the loop above ---------------------------------------------
+ * ldso_b200_optimize_finish: the newest keyframe's new evaluation point (setEvalPT(PRE_worldToCam, newStateZero): eval pose = current
+ * pose, state = state_zero = 0 except [6..7] = the current state[6..7]), setAdjointsF and setPrecalcValues for every pair, then
+ * linearizeAll(true) over the window's non-linearised residuals: linearize, applyRes(true), energy, setNewFrameEnergyTH, and per
+ * point the max relative baseline and the count of the residuals still active, per residual whether it is dropped
+ * (ef->dropResidual). The RMSE is sqrtf((float) (energy / (patternNum * resInA))) with the resInA of the last solve; the frame is
+ * lost when the energy is not finite. Asynchronous like gn_iterations_until; with fewer than 2 frames it launches nothing and
+ * get_finish reports zeros (optimize returns 0, FullSystem.cc:727-728). Single, unsharded contexts only.
+ * State rule: afterwards the device window still holds the dropped residuals and the null-space projector belongs to the old
+ * evaluation point. Every entry point that computes on the window returns LDSO_B200_ERR_STATE until the next set_window, and the
+ * solve entry points (optimize_begin, gn_iterations*, solve_system, do_step, gn_phase_a) also until the next set_frames --
+ * the order LDSO keeps (the next keyframe's insertFrame / makeIDX come first). marginalize_points needs set_window only.
+ * The getters keep working: get_frames returns the new adjoints and pair records, get_points / get_residuals the fixed linearisation. */
+int ldso_b200_optimize_finish(ldso_b200_ctx *ctx);
+/* Synchronises; any pointer may be NULL. res_state / res_dropped [nResiduals]; pt_relBS_max / pt_n_good [nPoints]: pt_relBS_max is 0
+ * for a point without an active residual. The caller applies maxRelBaseline = max(maxRelBaseline, pt_relBS_max) and
+ * numGoodResiduals += pt_n_good (host state the window does not carry), and removes the dropped residuals. newest_evalR (row-major),
+ * newest_evalT, newest_state_zero: the newest frame's new evaluation point. Readable until the next set_window or set_frames
+ * (LDSO_B200_ERR_STATE afterwards). */
+int ldso_b200_get_finish(ldso_b200_ctx *ctx, double *energy, float *rmse, int *is_lost, uint8_t *res_state, uint8_t *res_dropped,
+                         float *pt_relBS_max, int32_t *pt_n_good, double newest_evalR[9], double newest_evalT[3], double newest_state_zero[10]);
+/* What get_finish returns, for the one-call form below; any pointer may be NULL. */
+typedef struct ldso_b200_finish_out {
+    int *iterations_run;                 /* bodies the loop ran */
+    double *energy; float *rmse; int *is_lost;
+    uint8_t *res_state, *res_dropped;    /* [nResiduals] */
+    float *pt_relBS_max; int32_t *pt_n_good;     /* [nPoints] */
+    double *newest_evalR, *newest_evalT, *newest_state_zero;     /* [9], [3], [10] */
+} ldso_b200_finish_out;
+/* One keyframe's FullSystem::optimize from host buffers: optimize_from_host_until followed by optimize_finish. io's outputs are
+ * the loop's results exactly as optimize_from_host_until returns them; *out receives what get_finish returns. _full_submit /
+ * _full_wait split it like the pairs above and keep their two-context overlap. */
+int ldso_b200_optimize_from_host_full(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, int min_iterations, const ldso_b200_finish_out *out);
+int ldso_b200_optimize_from_host_full_submit(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, int min_iterations);
+int ldso_b200_optimize_from_host_full_wait(ldso_b200_ctx *ctx, const ldso_b200_fused_io *io, const ldso_b200_finish_out *out);
+
 /* Multi-GPU (SURVEY §8e): points are sharded over ranks (one context per GPU), frames/images replicated. A GN
  * iteration is split around the ONE collective: gn_phase_a(iteration) runs [solve + frame step of `iteration`
  * (skipped when iteration < 0 = the optimize() prologue)] + resubstitute/linearize/accumulate on this rank's

@@ -52,6 +52,11 @@ class FusedIOC(C.Structure):
                 ("pt_step", c_fp), ("pt_HdiF", c_fp), ("res_state", c_bp), ("res_new_state", c_bp), ("res_energy", c_fp)]
 
 
+class FinishOutC(C.Structure):
+    _fields_ = [("iterations_run", c_ip), ("energy", c_dp), ("rmse", c_fp), ("is_lost", c_ip), ("res_state", c_bp), ("res_dropped", c_bp),
+                ("pt_relBS_max", c_fp), ("pt_n_good", c_ip), ("newest_evalR", c_dp), ("newest_evalT", c_dp), ("newest_state_zero", c_dp)]
+
+
 class FrameStateC(C.Structure):
     _fields_ = [("evalR", C.c_double * 9), ("evalT", C.c_double * 3), ("state_zero", C.c_double * 10),
                 ("state", C.c_double * 10), ("ab_exposure", C.c_float), ("frameEnergyTH", C.c_float),
@@ -71,7 +76,8 @@ SYMBOLS = [
     "ldso_b200_solve_system", "ldso_b200_get_system", "ldso_b200_do_step", "ldso_b200_marginalize_points", "ldso_b200_marginalize_frame", "ldso_b200_calc_energies", "ldso_b200_accumulate", "ldso_b200_select_activation", "ldso_b200_init_calc_res", "ldso_b200_optimize_begin",
     "ldso_b200_gn_iterations", "ldso_b200_gn_iterations_until", "ldso_b200_get_iterations_run", "ldso_b200_get_until_form",
     "ldso_b200_optimize_iteration_budget", "ldso_b200_optimize_from_host_until", "ldso_b200_optimize_from_host_until_submit",
-    "ldso_b200_optimize_from_host_until_wait", "ldso_b200_optimize_from_host", "ldso_b200_optimize_from_host_submit", "ldso_b200_optimize_from_host_wait", "ldso_b200_reduce_buffer", "ldso_b200_set_shard", "ldso_b200_gn_phase_a",
+    "ldso_b200_optimize_from_host_until_wait", "ldso_b200_optimize_finish", "ldso_b200_get_finish",
+    "ldso_b200_optimize_from_host_full", "ldso_b200_optimize_from_host_full_submit", "ldso_b200_optimize_from_host_full_wait", "ldso_b200_optimize_from_host", "ldso_b200_optimize_from_host_submit", "ldso_b200_optimize_from_host_wait", "ldso_b200_reduce_buffer", "ldso_b200_set_shard", "ldso_b200_gn_phase_a",
     "ldso_b200_gn_phase_b", "ldso_b200_peer_export", "ldso_b200_peer_connect", "ldso_b200_peer_error", "ldso_b200_prefetch_results", "ldso_b200_get_energy", "ldso_b200_get_last_solution", "ldso_b200_get_points",
     "ldso_b200_get_residuals", "ldso_b200_get_frames", "ldso_b200_get_nullspace_projector", "ldso_b200_immature_init",
     "ldso_b200_trace_immature", "ldso_b200_optimize_immature", "ldso_b200_tracker_make_k",
@@ -358,6 +364,18 @@ class Context:
         self._chk(self.L.ldso_b200_get_until_form(self.ctx, C.byref(f)))
         return UNTIL_FORMS[f.value]
 
+    def optimize_finish(self):
+        """The end of FullSystem::optimize (FullSystem.cc:833-863) on the device: the newest frame's new evaluation point, the
+        adjoints and pair records, linearizeAll(true) with its per-point bookkeeping, the RMSE. Asynchronous; finish_results()
+        reads it back. Afterwards the window entry points need set_window, the solve entry points also set_frames."""
+        self._chk(self.L.ldso_b200_optimize_finish(self.ctx))
+
+    def finish_results(self):
+        """What ldso_b200_get_finish returns, as a dict of arrays."""
+        out = _finish_arrays(self.nP, self.nR)
+        self._chk(self.L.ldso_b200_get_finish(self.ctx, *_finish_ptrs(out)))
+        return _finish_scalars(out)
+
     def reduce_buffer(self):
         p = C.c_void_p()
         n = C.c_size_t()
@@ -613,6 +631,23 @@ Context.tracker_track_batch = Context._tracker_track_batch
 Context.posegraph_optimize = Context._posegraph_optimize
 
 
+def _finish_arrays(nP, nR):
+    return dict(energy=np.zeros(1), rmse=np.zeros(1, np.float32), is_lost=np.zeros(1, np.int32), res_state=np.zeros(nR, np.uint8),
+                res_dropped=np.zeros(nR, np.uint8), pt_relBS_max=np.zeros(nP, np.float32), pt_n_good=np.zeros(nP, np.int32),
+                newest_evalR=np.zeros((3, 3)), newest_evalT=np.zeros(3), newest_state_zero=np.zeros(10))
+
+
+def _finish_ptrs(o):
+    return (_d(o["energy"]), _f(o["rmse"]), _i(o["is_lost"]), _b(o["res_state"]), _b(o["res_dropped"]), _f(o["pt_relBS_max"]),
+            _i(o["pt_n_good"]), _d(o["newest_evalR"]), _d(o["newest_evalT"]), _d(o["newest_state_zero"]))
+
+
+def _finish_scalars(o):
+    o = dict(o)
+    o["energy"], o["rmse"], o["is_lost"] = float(o["energy"][0]), float(o["rmse"][0]), bool(o["is_lost"][0])
+    return o
+
+
 class StepIO:
     """Persistent host buffers + pre-built C argument blocks for one window, the way a C++ caller holds them: every
     call below is the bare C-ABI call on memory allocated once (no per-call numpy allocation or dtype conversion).
@@ -699,6 +734,34 @@ class StepIO:
         self.ctx.nF, self.ctx.nP, self.ctx.nR = self.nF, self.nP, self.nR
         self.iterations_run = n.value
         return self.out
+
+    def _finish_out(self):
+        if not hasattr(self, "_fo"):
+            self.finish = _finish_arrays(self.nP, self.nR)
+            self._fin_n = np.zeros(1, np.int32)
+            self._fo = FinishOutC(_i(self._fin_n), *_finish_ptrs(self.finish))
+        return C.byref(self._fo)
+
+    def _finished(self):
+        self.ctx.nF, self.ctx.nP, self.ctx.nR = self.nF, self.nP, self.nR
+        self.iterations_run = int(self._fin_n[0])
+        return self.out, _finish_scalars(self.finish)
+
+    def submit_full(self, iteration=0, max_iterations=6, min_iterations=1):
+        """ldso_b200_optimize_from_host_full_submit: the step with the exit and the finish, not waited for."""
+        self._prep(iteration, max_iterations)
+        self.ctx._chk(self.L.ldso_b200_optimize_from_host_full_submit(self.h, C.byref(self._io), int(min_iterations)))
+
+    def wait_full(self):
+        """ldso_b200_optimize_from_host_full_wait: (loop outputs, finish results)."""
+        self.ctx._chk(self.L.ldso_b200_optimize_from_host_full_wait(self.h, C.byref(self._io), self._finish_out()))
+        return self._finished()
+
+    def fused_full(self, iteration=0, max_iterations=6, min_iterations=1):
+        """ldso_b200_optimize_from_host_full: one keyframe's whole FullSystem::optimize as ONE call: (loop outputs, finish results)."""
+        self._prep(iteration, max_iterations)
+        self.ctx._chk(self.L.ldso_b200_optimize_from_host_full(self.h, C.byref(self._io), int(min_iterations), self._finish_out()))
+        return self._finished()
 
     def scalars(self):
         """(energy, canbreak) the last fused / submitted step returned"""

@@ -20,6 +20,7 @@
 #include "trace_types.h"
 #include "posegraph.cuh"
 #include "gn_loop.cuh"
+#include "finish.cuh"
 
 static_assert(K1_THREADS / 32 == MAXF, "phase B maps one warp to one target frame");
 
@@ -91,6 +92,13 @@ struct ldso_b200_ctx {
     int until_launches_per_body = 0; // kernels per body of the last WHILE-node launch, not yet in `launches`
     int *loop_dev = nullptr;         // k_gn_continue's parameters and counters (LOOP_*)
     int *loop_pin = nullptr;         // pinned: the host-driven form reads LOOP_CONT back here
+    // optimize_finish: per-point / per-residual outputs (window arrays) and the two scalars; fin_state 0 = nothing to read,
+    // 1 = the last finish had fewer than 2 frames (nothing ran, get_finish reports zeros), 2 = results on the device
+    FinishBufs fb = {};
+    int fin_state = 0;
+    // after optimize_finish the window still holds the dropped residuals and the null-space projector is stale: the window
+    // entry points wait for the next set_window, the solve entry points also for the next set_frames
+    bool fin_window_stale = false, fin_frames_stale = false;
     bool use_graph = true;
     bool use_pdl = true;             // programmatic dependent launch inside the GN iteration (env LDSO_B200_NO_PDL disables)
     bool pdl_now = false;            // set while launch_gn_body issues its four kernels
@@ -221,6 +229,7 @@ extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_lev
     ok = ok && cudaMalloc(&c->iteration_dev, sizeof(int)) == cudaSuccess;
     ok = ok && cudaMalloc(&c->loop_dev, sizeof(int) * LOOP_WORDS) == cudaSuccess;
     ok = ok && cudaMallocHost(&c->loop_pin, sizeof(int) * LOOP_WORDS) == cudaSuccess;
+    ok = ok && cudaMalloc(&c->fb.rmse, sizeof(float) + sizeof(int)) == cudaSuccess;
     // solve buffers: 4 + 1 + 1 + 1 matrices (n x n) and 6 vectors
     const size_t nn = (size_t) MAXN * MAXN;
     ok = ok && cudaMalloc(&c->solve_mem, sizeof(double) * (7 * nn + 8 * MAXN)) == cudaSuccess;
@@ -233,6 +242,7 @@ extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_lev
     cudaMemset(c->trk_counter, 0, sizeof(unsigned));
     cudaMemset(c->iteration_dev, 0, sizeof(int));
     cudaMemset(c->loop_dev, 0, sizeof(int) * LOOP_WORDS);
+    c->fb.is_lost = (int *) (c->fb.rmse + 1);
     cudaMemset(c->ws_dev, 0, sizeof(WinState));
     memset(c->ws_host, 0, sizeof(WinState));
     double *p = c->solve_mem;
@@ -299,6 +309,7 @@ extern "C" void ldso_b200_destroy(ldso_b200_ctx *c) {
     if (c->iteration_dev) cudaFree(c->iteration_dev);
     if (c->loop_dev) cudaFree(c->loop_dev);
     if (c->loop_pin) cudaFreeHost(c->loop_pin);
+    if (c->fb.rmse) cudaFree(c->fb.rmse);
     if (c->solve_mem) cudaFree(c->solve_mem);
     if (c->trk_partials) cudaFree(c->trk_partials);
     if (c->trk_counter) cudaFree(c->trk_counter);
@@ -472,6 +483,7 @@ static int alloc_window(ldso_b200_ctx *c, int nP, int nR) {
     rc |= dev_alloc(c, &d.res_proj, (size_t) nR * 16); rc |= dev_alloc(c, &d.res_cpt, (size_t) nR * 3);
     rc |= dev_alloc(c, &d.res_toZero, (size_t) nR * 8);
     rc |= dev_alloc(c, &c->pt_sel_dev, nP);
+    rc |= dev_alloc(c, &c->fb.pt_relBS_max, nP); rc |= dev_alloc(c, &c->fb.pt_n_good, nP); rc |= dev_alloc(c, &c->fb.res_dropped, nR);
     return rc ? LDSO_B200_ERR_CUDA : LDSO_B200_OK;
 }
 
@@ -540,12 +552,14 @@ extern "C" int ldso_b200_set_window(ldso_b200_ctx *c, const ldso_b200_window *wi
     { c->mirror_valid = false; c->results_inflight = false; c->sol_valid = false; c->mirror_full_valid = false; }
     c->solve_ready = false; c->restitch_ok = false;
     c->have_window = true;
+    c->fin_window_stale = false; c->fin_state = 0;
     return LDSO_B200_OK;
 }
 
 // work items, newest-frame slots, partial buffers: need both the window and nF
 static int build_derived(ldso_b200_ctx *c) {
     if (!c->have_window || !c->have_frames) return c->fail(LDSO_B200_ERR_STATE, "set_frames and set_window must both be called first");
+    if (c->fin_window_stale) return c->fail(LDSO_B200_ERR_STATE, "optimize_finish left dropped residuals in the window: call set_window first");
     if (!c->derived_dirty) return LDSO_B200_OK;
     DevWindow &d = c->d;
     const int nP = d.nP, nR = d.nR, nF = c->nF;
@@ -605,6 +619,12 @@ static int build_derived(ldso_b200_ctx *c) {
     d.items = items_dev; d.host_item_begin = hib_dev; d.res_newest_slot = slot_dev;
     c->derived_dirty = false;
     c->gn_graph_valid = false; c->until_graph_valid = false;
+    return LDSO_B200_OK;
+}
+
+// the solve entry points also need the null-space projector of the current evaluation points (set_frames after optimize_finish)
+static int check_solve_frames(ldso_b200_ctx *c) {
+    if (c->fin_frames_stale) return c->fail(LDSO_B200_ERR_STATE, "optimize_finish moved the newest evaluation point: call set_frames first");
     return LDSO_B200_OK;
 }
 
@@ -762,6 +782,8 @@ extern "C" int ldso_b200_set_frames(ldso_b200_ctx *c, int nFrames, const ldso_b2
     LAUNCH_CHECK(c);
     c->solve_ready = false; c->restitch_ok = false; c->select_pending = false;
     c->have_frames = true;
+    c->fin_frames_stale = false;
+    c->fin_state = 0;        // get_finish describes the frames the finish ran on, not these
     if (prev_nF != nF) c->derived_dirty = true;    // work items / newest-frame slots depend on nF only
     return LDSO_B200_OK;
 }
@@ -918,6 +940,7 @@ extern "C" int ldso_b200_solve_system(ldso_b200_ctx *c, int iteration, double *l
     if (!c) return LDSO_B200_ERR_ARG;
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
+    RET_IF(check_solve_frames(c));
     // records from the stored Jacobians: accumulateAF (mode 0); with linearized residuals in the window, accumulateLF's terms
     // (mode 1: res_toZeroF + J delta) ride in the same pass -- solveSystemF only ever uses HA + HL and the summed point terms
     RET_IF(launch_k1(c, K1F_ACCUMULATE | ((c->has_lin ? 3 : 0) << K1F_MODE_SHIFT)));
@@ -995,6 +1018,7 @@ extern "C" int ldso_b200_do_step(ldso_b200_ctx *c, int *canbreak) {
     if (!c) return LDSO_B200_ERR_ARG;
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
+    RET_IF(check_solve_frames(c));
     k_sum_nid<<<1, 256, 0, c->stream>>>(c->d, c->ws_dev);
     LAUNCH_CHECK(c);
     RET_IF(launch_k3(c, K3F_STEP));
@@ -1365,6 +1389,7 @@ extern "C" int ldso_b200_optimize_begin(ldso_b200_ctx *c, double *energy_out) {
     if (!c) return LDSO_B200_ERR_ARG;
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
+    RET_IF(check_solve_frames(c));
     RET_IF(clear_select(c));
     RET_IF(launch_k1(c, K1_FUSED | K1F_RESET_OOB));
     RET_IF(launch_k2a(c, 1));
@@ -1405,6 +1430,7 @@ extern "C" int ldso_b200_gn_iterations(ldso_b200_ctx *c, int first_iteration, in
     if (c->multi && !c->peers_connected) return c->fail(LDSO_B200_ERR_STATE, "sharded context without peer exchange: use gn_phase_a / all-reduce / gn_phase_b, or peer_export + peer_connect");
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
+    RET_IF(check_solve_frames(c));
     RET_IF(ensure_solve_ready(c));
     RET_IF(set_iteration(c, first_iteration));     // K3 reads the iteration number from device memory and increments it
     if (c->use_graph && c->d.nItems > 0) {
@@ -1535,6 +1561,7 @@ extern "C" int ldso_b200_gn_iterations_until(ldso_b200_ctx *c, int first_iterati
     if (c->multi && !c->peers_connected) return c->fail(LDSO_B200_ERR_STATE, "sharded context without peer exchange: use gn_phase_a / all-reduce / gn_phase_b, or peer_export + peer_connect");
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
+    RET_IF(check_solve_frames(c));
     RET_IF(ensure_solve_ready(c));
     const int params[LOOP_CONT] = {max_iterations, min_iterations, 0};      // LOOP_MAX, LOOP_MIN, LOOP_RUN
     CUDA_CHECK_RET(c, cudaMemcpyAsync(c->loop_dev, params, sizeof(params), cudaMemcpyHostToDevice, c->stream));
@@ -1652,6 +1679,94 @@ extern "C" int ldso_b200_optimize_from_host_until(ldso_b200_ctx *c, const ldso_b
     return ldso_b200_optimize_from_host_until_wait(c, io, iterations_run);
 }
 
+// ---- the end of FullSystem::optimize (FullSystem.cc:833-863)
+// k_finish_frames (new evaluation point of the newest frame, adjoints, pair records) -> K1 (linearize + applyRes(true), as
+// linearize_all(1)) -> K2a / K2b (energy, setNewFrameEnergyTH) -> k_finish_points (relBS, numGoodResiduals, dropped residuals)
+// -> k_finish_tail (RMSE, lost). The pending setNewFrameEnergyTH of the loop's last linearisation runs first: LDSO's last
+// linearizeAll(false) finished it before the epilogue began.
+extern "C" int ldso_b200_optimize_finish(ldso_b200_ctx *c) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    if (c->multi) return c->fail(LDSO_B200_ERR_STATE, "optimize_finish runs on a single, unsharded context");
+    cudaSetDevice(c->device);
+    RET_IF(build_derived(c));
+    if (c->nF < 2) { c->fin_state = 1; return LDSO_B200_OK; }     // FullSystem.cc:727-728: optimize returns 0 before anything runs
+    RET_IF(flush_select(c));
+    k_finish_frames<<<1, 128, 0, c->stream>>>(c->ws_dev);
+    LAUNCH_CHECK(c);
+    RET_IF(launch_k1(c, K1F_LINEARIZE | K1F_STORE_J | K1F_APPLY_RES));       // as linearize_all(1): get_residuals reads its Jacobians
+    RET_IF(launch_k2a(c, 0));
+    RET_IF(launch_k2b(c, 0, 1, 0));
+    if (c->d.nP > 0) {
+        k_finish_points<<<(c->d.nP + 127) / 128, 128, 0, c->stream>>>(c->d, (const WinState *) c->ws_dev, c->fb);
+        LAUNCH_CHECK(c);
+    }
+    k_finish_tail<<<1, 32, 0, c->stream>>>((const WinState *) c->ws_dev, c->fb);
+    LAUNCH_CHECK(c);
+    c->fin_state = 2;
+    c->fin_window_stale = true; c->fin_frames_stale = true;
+    c->solve_ready = false; c->restitch_ok = false;
+    c->evalpt_key.clear();      // the device adjoints now belong to the new evaluation point: the next set_frames recomputes them
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_get_finish(ldso_b200_ctx *c, double *energy, float *rmse, int *is_lost, uint8_t *res_state, uint8_t *res_dropped,
+                                    float *pt_relBS_max, int32_t *pt_n_good, double newest_evalR[9], double newest_evalT[3],
+                                    double newest_state_zero[10]) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    if (c->fin_state == 0 || !c->have_window || !c->have_frames) return c->fail(LDSO_B200_ERR_STATE, "no optimize_finish to read");
+    cudaSetDevice(c->device);
+    const size_t nP = c->d.nP, nR = c->d.nR;
+    FrameDev fr;
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(&fr, &c->ws_dev->fr[c->nF - 1], sizeof(FrameDev), cudaMemcpyDeviceToHost, c->stream));
+    if (c->fin_state == 2) {
+        D2H(energy, &c->ws_dev->energy, sizeof(double));
+        D2H(rmse, c->fb.rmse, sizeof(float));
+        D2H(is_lost, c->fb.is_lost, sizeof(int));
+        D2H(res_state, c->d.res_state, nR);
+        D2H(res_dropped, c->fb.res_dropped, nR);
+        D2H(pt_relBS_max, c->fb.pt_relBS_max, 4 * nP);
+        D2H(pt_n_good, c->fb.pt_n_good, 4 * nP);
+    } else {
+        if (energy) *energy = 0.0;
+        if (rmse) *rmse = 0.f;
+        if (is_lost) *is_lost = 0;
+        D2H(res_state, c->d.res_state, nR);
+        if (res_dropped) memset(res_dropped, 0, nR);
+        if (pt_relBS_max) memset(pt_relBS_max, 0, 4 * nP);
+        if (pt_n_good) memset(pt_n_good, 0, 4 * nP);
+    }
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    if (newest_evalR) memcpy(newest_evalR, fr.evalR, sizeof(fr.evalR));
+    if (newest_evalT) memcpy(newest_evalT, fr.evalT, sizeof(fr.evalT));
+    if (newest_state_zero) memcpy(newest_state_zero, fr.state_zero, sizeof(fr.state_zero));
+    return LDSO_B200_OK;
+}
+
+// optimize_from_host_until + optimize_finish. io's outputs are the loop's results (read back into pinned staging before the finish
+// runs, as optimize_from_host_until returns them); `out` receives what get_finish returns.
+extern "C" int ldso_b200_optimize_from_host_full_submit(ldso_b200_ctx *c, const ldso_b200_fused_io *io, int min_iterations) {
+    RET_IF(submit_impl(c, io, true, min_iterations));
+    RET_IF(ldso_b200_optimize_finish(c));
+    // the finish's launches do not touch what the prefetch queued before them: keep waiting on that copy
+    c->results_inflight = true;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_optimize_from_host_full_wait(ldso_b200_ctx *c, const ldso_b200_fused_io *io, const ldso_b200_finish_out *out) {
+    if (!c || !out) return LDSO_B200_ERR_ARG;
+    RET_IF(ldso_b200_optimize_from_host_until_wait(c, io, out->iterations_run));
+    // the mirror holds the loop's results, the device the finish's
+    { c->mirror_valid = false; c->sol_valid = false; c->mirror_full_valid = false; }
+    return ldso_b200_get_finish(c, out->energy, out->rmse, out->is_lost, out->res_state, out->res_dropped, out->pt_relBS_max, out->pt_n_good,
+                                out->newest_evalR, out->newest_evalT, out->newest_state_zero);
+}
+
+extern "C" int ldso_b200_optimize_from_host_full(ldso_b200_ctx *c, const ldso_b200_fused_io *io, int min_iterations, const ldso_b200_finish_out *out) {
+    if (!c || !out) return LDSO_B200_ERR_ARG;
+    RET_IF(ldso_b200_optimize_from_host_full_submit(c, io, min_iterations));
+    return ldso_b200_optimize_from_host_full_wait(c, io, out);
+}
+
 extern "C" int ldso_b200_reduce_buffer(ldso_b200_ctx *c, void **buf_dev, size_t *n_doubles) {
     if (!c || !buf_dev || !n_doubles) return LDSO_B200_ERR_ARG;
     cudaSetDevice(c->device);
@@ -1739,6 +1854,7 @@ extern "C" int ldso_b200_gn_phase_a(ldso_b200_ctx *c, int iteration) {
     if (!c) return LDSO_B200_ERR_ARG;
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
+    RET_IF(check_solve_frames(c));
     RET_IF(clear_select(c));
     if (iteration < 0) {
         RET_IF(launch_k1(c, K1_FUSED | K1F_RESET_OOB));

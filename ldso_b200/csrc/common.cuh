@@ -125,6 +125,7 @@ struct WinState {
     // scalars produced on the device
     double energy;                    // last linearizeAll energy (lastEnergyP)
     int resInA;
+    int resInA_solved;                // resInA of the system the last K3 solve used (EnergyFunctional::resInA after solveSystemF)
     int canbreak;
     int iteration_count;
     float sumNID, numID;
