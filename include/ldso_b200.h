@@ -95,6 +95,37 @@ int ldso_b200_make_images(ldso_b200_ctx *ctx, int slot, const float *color);
 /* read a level back as (I,dx,dy) AoS — tests only */
 int ldso_b200_download_frame_level(ldso_b200_ctx *ctx, int slot, int lvl, float *dIp_out);
 
+/* ---- raw camera frames: LDSO's per-frame undistortion on the device ------------------------------------
+ * Undistort::undistort<T> (src/frontend/Undistort.cc:357-457) with PhotometricUndistorter::processFrame<T> (:189-227) in front
+ * of makeImages: the raw 8- or 16-bit frame goes through the inverse response G (and the vignette in mode 2) and is bilinearly
+ * remapped onto the rectified grid in one kernel, and the pyramid is built from the result as ldso_b200_make_images does.
+ * The tables are the ones LDSO's Undistort built from its calibration files. Every output pixel equals the reference's bit for bit,
+ * except where the reference reads past the end of its raw buffer (a remap offset of exactly (hOrg-1)*wOrg or (hOrg-1)*wOrg - 1):
+ * those taps read 0 here. The benchmark noise settings (benchmark_varNoise, benchmark_varBlurNoise) are not supported. */
+typedef struct ldso_b200_undistort_calib {
+    int wOrg, hOrg;                 /* raw frame size (Undistort::getOriginalSize) */
+    int w, h;                       /* rectified size (Undistort::getSize): must be the context's w x h */
+    const float *remapX, *remapY;   /* w*h each (Undistort::remapX / remapY); both NULL = passthrough (needs wOrg x hOrg == w x h) */
+    const float *G;                 /* PhotometricUndistorter::G, g_entries floats (256 or 65536); NULL = no valid calibration
+                                     * (getG() == 0): every frame takes the factor path */
+    int g_entries;
+    const float *vignetteMapInv;    /* wOrg*hOrg floats; needed when G is given and photometric_mode == 2 */
+    int photometric_mode;           /* setting_photometricCalibration: 0, 1 or 2 */
+    int use_exposure;               /* setting_useExposure */
+} ldso_b200_undistort_calib;
+/* Copies the tables to the device (synchronising the context's stream). LDSO_B200_ERR_ARG for an inconsistent calibration: a
+ * rectified size other than the context's, one of remapX / remapY missing, passthrough with wOrg x hOrg != w x h, g_entries
+ * other than 256 / 65536 with G, photometric_mode 2 with G but no vignetteMapInv, photometric_mode outside 0..2. */
+int ldso_b200_set_undistort(ldso_b200_ctx *ctx, const ldso_b200_undistort_calib *calib);
+/* One raw frame (wOrg*hOrg pixels of bytes_per_pixel = 1 or 2 bytes) -> rectified irradiance -> the pyramid of `slot`, as
+ * undistort<T>(raw, exposure, 0, factor) followed by makeImages. *exposure_time_out (may be NULL) gets processFrame's exposure
+ * time: `exposure`, or 1 when use_exposure == 0. Asynchronous like ldso_b200_make_images; `raw` must stay valid until the next
+ * synchronising call on the context. LDSO_B200_ERR_STATE before any set_undistort; LDSO_B200_ERR_ARG for a NULL raw, a
+ * bytes_per_pixel other than 1 / 2, or a 16-bit frame with a 256-entry G. The level-0 image comes back through
+ * ldso_b200_download_frame_level. */
+int ldso_b200_undistort_frame(ldso_b200_ctx *ctx, int slot, const void *raw, int bytes_per_pixel, float exposure, float factor,
+                              float *exposure_time_out);
+
 /* ---- the optimisation window ---------------------------------------------------------------------------
  * Flattened EnergyFunctional::allPoints (EnergyFunctional.cc:385-401, points ordered by host keyframe as
  * makeIDX produces them) with each point's PointHessian::residuals list (CSR). */

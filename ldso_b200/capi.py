@@ -67,11 +67,16 @@ FRAME_DTYPE = np.dtype([("evalR", "<f8", 9), ("evalT", "<f8", 3), ("state_zero",
                         ("ab_exposure", "<f4"), ("frameEnergyTH", "<f4"), ("frame_id", "<i4"), ("image_slot", "<i4")])
 assert FRAME_DTYPE.itemsize == C.sizeof(FrameStateC)
 
+class UndistortCalibC(C.Structure):
+    _fields_ = [("wOrg", C.c_int), ("hOrg", C.c_int), ("w", C.c_int), ("h", C.c_int), ("remapX", c_fp), ("remapY", c_fp),
+                ("G", c_fp), ("g_entries", C.c_int), ("vignetteMapInv", c_fp), ("photometric_mode", C.c_int), ("use_exposure", C.c_int)]
+
+
 # every symbol include/ldso_b200.h declares (tests check the shared object exports all of them)
 SYMBOLS = [
     "ldso_b200_default_settings", "ldso_b200_create", "ldso_b200_destroy", "ldso_b200_last_error", "ldso_b200_set_stream",
     "ldso_b200_synchronize", "ldso_b200_launch_count", "ldso_b200_kernel_times", "ldso_b200_upload_frame", "ldso_b200_make_images",
-    "ldso_b200_download_frame_level", "ldso_b200_set_window", "ldso_b200_set_frames", "ldso_b200_set_marg_prior",
+    "ldso_b200_download_frame_level", "ldso_b200_set_undistort", "ldso_b200_undistort_frame", "ldso_b200_set_window", "ldso_b200_set_frames", "ldso_b200_set_marg_prior",
     "ldso_b200_get_marg_prior", "ldso_b200_linearize_all", "ldso_b200_apply_res", "ldso_b200_backup_state",
     "ldso_b200_solve_system", "ldso_b200_get_system", "ldso_b200_do_step", "ldso_b200_marginalize_points", "ldso_b200_marginalize_frame", "ldso_b200_calc_energies", "ldso_b200_accumulate", "ldso_b200_select_activation", "ldso_b200_init_calc_res", "ldso_b200_optimize_begin",
     "ldso_b200_gn_iterations", "ldso_b200_gn_iterations_until", "ldso_b200_get_iterations_run", "ldso_b200_get_until_form",
@@ -104,6 +109,8 @@ def load():
         L.ldso_b200_launch_count.restype = C.c_longlong
         L.ldso_b200_launch_count.argtypes = [C.c_void_p]
         L.ldso_b200_set_stream.argtypes = [C.c_void_p, C.c_void_p]
+        L.ldso_b200_set_undistort.argtypes = [C.c_void_p, C.POINTER(UndistortCalibC)]
+        L.ldso_b200_undistort_frame.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_float, c_fp]
         for name in SYMBOLS:
             fn = getattr(L, name)
             if name not in ("ldso_b200_create", "ldso_b200_destroy", "ldso_b200_last_error", "ldso_b200_launch_count",
@@ -215,6 +222,40 @@ class Context:
         out = np.zeros((self.h >> lvl, self.w >> lvl, 3), np.float32)
         self._chk(self.L.ldso_b200_download_frame_level(self.ctx, int(slot), int(lvl), _f(out)))
         return out
+
+    # ---- raw camera frames (undistortion on the device)
+    def set_undistort(self, wOrg, hOrg, remapX=None, remapY=None, G=None, vignetteMapInv=None, photometric_mode=2, use_exposure=True):
+        """ldso_b200_set_undistort with LDSO's Undistort tables: remapX / remapY (h x w, None = passthrough), G (256 or 65536
+        entries, None = no valid photometric calibration), vignetteMapInv (hOrg x wOrg), setting_photometricCalibration and
+        setting_useExposure. The arrays are copied to the device before this returns."""
+        arrs = {}
+        for name, a, n in (("remapX", remapX, self.w * self.h), ("remapY", remapY, self.w * self.h), ("G", G, None),
+                           ("vignetteMapInv", vignetteMapInv, int(wOrg) * int(hOrg))):
+            if a is None:
+                continue
+            a = np.ascontiguousarray(a, np.float32).reshape(-1)
+            if n is not None and a.size != n:
+                raise ValueError(f"{name} has {a.size} entries, expected {n}")
+            arrs[name] = a
+        c = UndistortCalibC(int(wOrg), int(hOrg), self.w, self.h, _f(arrs.get("remapX")), _f(arrs.get("remapY")), _f(arrs.get("G")),
+                            int(arrs["G"].size) if "G" in arrs else 0, _f(arrs.get("vignetteMapInv")), int(photometric_mode),
+                            int(bool(use_exposure)))
+        self._chk(self.L.ldso_b200_set_undistort(self.ctx, C.byref(c)))
+        self._ud_size = (int(hOrg), int(wOrg))
+
+    def undistort_frame(self, slot, raw, exposure, factor=1.0) -> float:
+        """ldso_b200_undistort_frame: one raw uint8 / uint16 frame (hOrg x wOrg) -> rectified irradiance -> slot's pyramid.
+        Returns the frame's exposure time as processFrame sets it (exposure, or 1 without use_exposure)."""
+        raw = np.ascontiguousarray(raw)
+        if raw.dtype not in (np.uint8, np.uint16):
+            raise ValueError("raw must be uint8 or uint16")
+        if getattr(self, "_ud_size", None) is not None and raw.size != self._ud_size[0] * self._ud_size[1]:
+            raise ValueError(f"raw has {raw.size} pixels, expected {self._ud_size[0]} x {self._ud_size[1]}")
+        e = C.c_float(0)
+        self._keep_raw = raw      # valid until the next synchronising call
+        self._chk(self.L.ldso_b200_undistort_frame(self.ctx, int(slot), raw.ctypes.data_as(C.c_void_p), raw.itemsize, float(exposure),
+                                                   float(factor), C.byref(e)))
+        return float(e.value)
 
     # ---- window
     def set_frames(self, Rcw, tcw, state_zero, state, ab_exposure, frame_id, slots, K_scaled, K_zero=None,

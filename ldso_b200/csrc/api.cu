@@ -21,6 +21,7 @@
 #include "posegraph.cuh"
 #include "gn_loop.cuh"
 #include "finish.cuh"
+#include "undistort.cuh"
 
 static_assert(K1_THREADS / 32 == MAXF, "phase B maps one warp to one target frame");
 
@@ -40,6 +41,14 @@ struct ldso_b200_ctx {
     float *scratch = nullptr;          // upload staging (w*h*3 floats)
     cudaEvent_t copy_done = nullptr, frames_copied = nullptr;
     size_t scratch_floats = 0;
+    // per-frame undistortion (set_undistort / undistort_frame): device tables, the raw frame buffer (wOrg*hOrg + wOrg + 1 pixels of
+    // 2 bytes, zero behind the frame) and its pinned staging copy
+    bool have_undistort = false;
+    ldso_b200_undistort_calib ud = {};     // the pointers in it are the device copies
+    float2 *ud_remap = nullptr;
+    float *ud_G = nullptr, *ud_vinv = nullptr;
+    void *ud_raw = nullptr, *ud_pin = nullptr;
+    cudaEvent_t ud_copied = nullptr;       // the staging buffer has been read by the last frame's copy
 
     // window
     DevWindow d;
@@ -264,6 +273,17 @@ extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_lev
     return c;
 }
 
+static void free_undistort(ldso_b200_ctx *c) {
+    if (c->ud_remap) cudaFree(c->ud_remap);
+    if (c->ud_G) cudaFree(c->ud_G);
+    if (c->ud_vinv) cudaFree(c->ud_vinv);
+    if (c->ud_raw) cudaFree(c->ud_raw);
+    if (c->ud_pin) cudaFreeHost(c->ud_pin);
+    if (c->ud_copied) cudaEventDestroy(c->ud_copied);
+    c->ud_remap = nullptr; c->ud_G = c->ud_vinv = nullptr; c->ud_raw = c->ud_pin = nullptr; c->ud_copied = nullptr;
+    c->have_undistort = false;
+}
+
 static void free_derived(ldso_b200_ctx *c) {
     for (void *p : c->derived_allocs) cudaFree(p);
     c->derived_allocs.clear();
@@ -297,6 +317,7 @@ extern "C" void ldso_b200_destroy(ldso_b200_ctx *c) {
     if (c->cd_tot) cudaFree(c->cd_tot);
     if (c->cd_in) cudaFree(c->cd_in);
     if (c->scratch) cudaFree(c->scratch);
+    free_undistort(c);
     if (c->ws_dev) cudaFree(c->ws_dev);
     if (c->ws_host) cudaFreeHost(c->ws_host);
     if (c->sol_host) cudaFreeHost(c->sol_host);
@@ -380,6 +401,17 @@ extern "C" int ldso_b200_upload_frame(ldso_b200_ctx *c, int slot, const float *c
     return LDSO_B200_OK;
 }
 
+// FrameHessian::makeImages on the device from the w*h irradiance image in c->scratch into slot's pyramid (ensure_slot done)
+static int pyramid_from_scratch(ldso_b200_ctx *c, int slot) {
+    for (int l = 0; l < c->levels; l++) {
+        const int npx = c->lw[l] * c->lh[l];
+        k_pyr_level<<<(npx + 255) / 256, 256, 0, c->stream>>>(c->scratch, l == 0 ? nullptr : c->img[slot][l - 1], c->img[slot][l],
+                                                                c->lw[l], c->lh[l], l == 0 ? 0 : c->lw[l - 1]);
+        LAUNCH_CHECK(c);
+    }
+    return LDSO_B200_OK;
+}
+
 static int make_images_impl(ldso_b200_ctx *c, int slot, const float *color, bool wait_copy) {
     if (!c || !color) return LDSO_B200_ERR_ARG;
     cudaSetDevice(c->device);
@@ -388,17 +420,86 @@ static int make_images_impl(ldso_b200_ctx *c, int slot, const float *color, bool
     CUDA_CHECK_RET(c, cudaMemcpyAsync(c->scratch, color, sizeof(float) * c->w * c->h, cudaMemcpyHostToDevice, c->stream));
     if (!c->copy_done) CUDA_CHECK_RET(c, cudaEventCreateWithFlags(&c->copy_done, cudaEventDisableTiming));
     CUDA_CHECK_RET(c, cudaEventRecord(c->copy_done, c->stream));
-    for (int l = 0; l < c->levels; l++) {
-        const int npx = c->lw[l] * c->lh[l];
-        k_pyr_level<<<(npx + 255) / 256, 256, 0, c->stream>>>(c->scratch, l == 0 ? nullptr : c->img[slot][l - 1], c->img[slot][l],
-                                                                c->lw[l], c->lh[l], l == 0 ? 0 : c->lw[l - 1]);
-        LAUNCH_CHECK(c);
-    }
+    RET_IF(pyramid_from_scratch(c, slot));
     // the caller's buffer is free once the copy has landed; the pyramid kernels keep running asynchronously
     if (wait_copy) CUDA_CHECK_RET(c, cudaEventSynchronize(c->copy_done));
     return LDSO_B200_OK;
 }
 extern "C" int ldso_b200_make_images(ldso_b200_ctx *c, int slot, const float *color) { return make_images_impl(c, slot, color, true); }
+
+// ---------------------------------------------------------------------------------------------- undistortion (undistort.cuh)
+extern "C" int ldso_b200_set_undistort(ldso_b200_ctx *c, const ldso_b200_undistort_calib *u) {
+    if (!c || !u) return LDSO_B200_ERR_ARG;
+    if (u->wOrg <= 0 || u->hOrg <= 0) return c->fail(LDSO_B200_ERR_ARG, "set_undistort: wOrg and hOrg must be positive");
+    if ((long long) u->wOrg * u->hOrg + u->wOrg + 1 > (1LL << 30)) return c->fail(LDSO_B200_ERR_ARG, "set_undistort: raw frame too large");
+    if (u->w != c->w || u->h != c->h) return c->fail(LDSO_B200_ERR_ARG, "set_undistort: the rectified size must be the context's w x h");
+    if ((u->remapX == nullptr) != (u->remapY == nullptr)) return c->fail(LDSO_B200_ERR_ARG, "set_undistort: remapX and remapY go together");
+    if (!u->remapX && (u->wOrg != c->w || u->hOrg != c->h))
+        return c->fail(LDSO_B200_ERR_ARG, "set_undistort: passthrough (no remap) needs wOrg x hOrg == the context's w x h");
+    if (u->photometric_mode < 0 || u->photometric_mode > 2) return c->fail(LDSO_B200_ERR_ARG, "set_undistort: photometric_mode must be 0, 1 or 2");
+    if (u->G && u->g_entries != 256 && u->g_entries != 65536) return c->fail(LDSO_B200_ERR_ARG, "set_undistort: g_entries must be 256 or 65536");
+    if (u->G && u->photometric_mode == 2 && !u->vignetteMapInv)
+        return c->fail(LDSO_B200_ERR_ARG, "set_undistort: photometric_mode 2 with a valid G needs vignetteMapInv");
+    cudaSetDevice(c->device);
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    free_undistort(c);
+    const size_t nOrg = (size_t) u->wOrg * u->hOrg, n = (size_t) c->w * c->h;
+    CUDA_CHECK_RET(c, cudaMalloc(&c->ud_raw, 2 * (nOrg + u->wOrg + 1)));
+    CUDA_CHECK_RET(c, cudaMemset(c->ud_raw, 0, 2 * (nOrg + u->wOrg + 1)));     // the zero pixels behind the frame stay zero
+    CUDA_CHECK_RET(c, cudaMallocHost(&c->ud_pin, 2 * nOrg));
+    CUDA_CHECK_RET(c, cudaEventCreateWithFlags(&c->ud_copied, cudaEventDisableTiming));
+    if (u->remapX) {
+        std::vector<float2> rm(n);
+        for (size_t i = 0; i < n; i++) rm[i] = make_float2(u->remapX[i], u->remapY[i]);
+        CUDA_CHECK_RET(c, cudaMalloc(&c->ud_remap, sizeof(float2) * n));
+        CUDA_CHECK_RET(c, cudaMemcpy(c->ud_remap, rm.data(), sizeof(float2) * n, cudaMemcpyHostToDevice));
+    }
+    if (u->G) {
+        CUDA_CHECK_RET(c, cudaMalloc(&c->ud_G, sizeof(float) * u->g_entries));
+        CUDA_CHECK_RET(c, cudaMemcpy(c->ud_G, u->G, sizeof(float) * u->g_entries, cudaMemcpyHostToDevice));
+    }
+    if (u->vignetteMapInv) {
+        CUDA_CHECK_RET(c, cudaMalloc(&c->ud_vinv, sizeof(float) * nOrg));
+        CUDA_CHECK_RET(c, cudaMemcpy(c->ud_vinv, u->vignetteMapInv, sizeof(float) * nOrg, cudaMemcpyHostToDevice));
+    }
+    c->ud = *u;
+    c->ud.remapX = c->ud.remapY = nullptr;
+    c->ud.G = c->ud_G;
+    c->ud.vignetteMapInv = c->ud_vinv;
+    c->have_undistort = true;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_undistort_frame(ldso_b200_ctx *c, int slot, const void *raw, int bytes_per_pixel, float exposure, float factor,
+                                         float *exposure_time_out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    if (!c->have_undistort) return c->fail(LDSO_B200_ERR_STATE, "undistort_frame: call set_undistort first");
+    if (!raw) return c->fail(LDSO_B200_ERR_ARG, "undistort_frame: raw is NULL");
+    if (bytes_per_pixel != 1 && bytes_per_pixel != 2) return c->fail(LDSO_B200_ERR_ARG, "undistort_frame: bytes_per_pixel must be 1 or 2");
+    if (bytes_per_pixel == 2 && c->ud.G && c->ud.g_entries < 65536)
+        return c->fail(LDSO_B200_ERR_ARG, "undistort_frame: a 16-bit frame needs a 65536-entry G");
+    cudaSetDevice(c->device);
+    RET_IF(ensure_slot(c, slot));
+    const size_t bytes = (size_t) bytes_per_pixel * c->ud.wOrg * c->ud.hOrg;
+    // the staging buffer is free once the previous frame's copy has read it
+    CUDA_CHECK_RET(c, cudaEventSynchronize(c->ud_copied));
+    memcpy(c->ud_pin, raw, bytes);
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->ud_raw, c->ud_pin, bytes, cudaMemcpyHostToDevice, c->stream));
+    CUDA_CHECK_RET(c, cudaEventRecord(c->ud_copied, c->stream));
+    UndistortArgs a;
+    a.remap = c->ud_remap; a.G = c->ud_G; a.vinv = c->ud_vinv;
+    a.wOrg = c->ud.wOrg; a.hOrg = c->ud.hOrg; a.w = c->w; a.h = c->h;
+    a.use_G = c->ud_G != nullptr && !(exposure <= 0) && c->ud.photometric_mode != 0;      // processFrame's branch (Undistort.cc:197)
+    a.mode2 = c->ud.photometric_mode == 2;
+    a.factor = factor;
+    const int npx = c->w * c->h;
+    if (bytes_per_pixel == 1) k_undistort<uint8_t><<<(npx + 255) / 256, 256, 0, c->stream>>>((const uint8_t *) c->ud_raw, a, c->scratch);
+    else k_undistort<uint16_t><<<(npx + 255) / 256, 256, 0, c->stream>>>((const uint16_t *) c->ud_raw, a, c->scratch);
+    LAUNCH_CHECK(c);
+    RET_IF(pyramid_from_scratch(c, slot));
+    if (exposure_time_out) *exposure_time_out = c->ud.use_exposure ? exposure : 1.f;
+    return LDSO_B200_OK;
+}
 
 extern "C" int ldso_b200_download_frame_level(ldso_b200_ctx *c, int slot, int lvl, float *out) {
     if (!c || !out || slot < 0 || slot >= NSLOTS || lvl < 0 || lvl >= c->levels || !c->img[slot][lvl]) return LDSO_B200_ERR_ARG;
