@@ -126,6 +126,37 @@ int ldso_b200_set_undistort(ldso_b200_ctx *ctx, const ldso_b200_undistort_calib 
 int ldso_b200_undistort_frame(ldso_b200_ctx *ctx, int slot, const void *raw, int bytes_per_pixel, float exposure, float factor,
                               float *exposure_time_out);
 
+/* ---- keyframe corners: LDSO's FeatureDetector::DetectCorners on the device -----------------------------
+ * FeatureDetector::DetectCorners(nFeatures, frame) (src/frontend/FeatureDetector.cc:34-130; setting_pointSelection == 1) on level 0
+ * of a slot's pyramid: the grid of cells, per cell the pixels whose absSquaredGrad (formed as makeImages forms it, with the gamma
+ * weight of B) exceeds max(0.5 * maxGrad, 5), their Shi-Tomasi scores, the best of them per cell, the corner threshold, the
+ * suppression of corners closer than 5 pixels, and IC_Angle and the ORB descriptor (ComputeDescriptor) of every corner. Features come
+ * in the reference's order. Two places where the reference's result depends on its libraries follow a fixed rule here (DESIGN.md
+ * "Keyframe corners"): within a cell, equal scores and NaN scores keep push order (x outer, y inner) and NaNs come after every
+ * number (std::sort is not stable); atan2f / cosf / sinf are evaluated in double and rounded to float. */
+typedef struct ldso_b200_features {
+    int capacity;                   /* entries the arrays below hold (at least ldso_b200_feature_capacity(w, h, nFeatures)) */
+    int n;                          /* out: number of features (frame->features.size()) */
+    float *u, *v;                   /* Feature::uv */
+    float *score;                   /* Feature::score (Shi-Tomasi) */
+    uint8_t *is_corner;             /* Feature::isCorner */
+    float *angle;                   /* Feature::angle (0 for a non-corner) */
+    uint8_t *descriptor;            /* Feature::descriptor, 32 bytes per feature (zero for a non-corner) */
+    int n_corners;                  /* out: DetectCorners' return value */
+} ldso_b200_features;
+/* ldso::bit_pattern_31_ (256 x 4 ints, FeatureDetector.cc), copied to the device; once per context, before detect_corners. */
+int ldso_b200_set_orb_pattern(ldso_b200_ctx *ctx, const int32_t pattern[1024]);
+/* The most features DetectCorners can return for a w x h image and nFeatures (cells x features per cell); LDSO_B200_ERR_ARG for
+ * nFeatures <= 0, a density whose gridsize is 0, or a grid whose angle / descriptor footprints can leave the image (the reference
+ * reads outside its buffer there; at 640 x 480 densities below about 320). Needs no context. */
+int ldso_b200_feature_capacity(int w, int h, int nFeatures);
+/* DetectCorners on the image in `slot` (filled by make_images, undistort_frame or upload_frame) with CalibHessian::B (256 floats, or
+ * NULL for the identity response). Runs on the context's stream after the work queued there, and returns with the results in *out:
+ * one device-to-host copy and one synchronise. LDSO_B200_ERR_STATE before set_orb_pattern; LDSO_B200_ERR_ARG for a slot out of range
+ * or never filled, a missing output array, a configuration ldso_b200_feature_capacity refuses, or a capacity below it. The features'
+ * ImmaturePoints come from ldso_b200_immature_init on the same slot. */
+int ldso_b200_detect_corners(ldso_b200_ctx *ctx, int slot, int nFeatures, const float *B, ldso_b200_features *out);
+
 /* ---- the optimisation window ---------------------------------------------------------------------------
  * Flattened EnergyFunctional::allPoints (EnergyFunctional.cc:385-401, points ordered by host keyframe as
  * makeIDX produces them) with each point's PointHessian::residuals list (CSR). */

@@ -72,11 +72,17 @@ class UndistortCalibC(C.Structure):
                 ("G", c_fp), ("g_entries", C.c_int), ("vignetteMapInv", c_fp), ("photometric_mode", C.c_int), ("use_exposure", C.c_int)]
 
 
+class FeaturesC(C.Structure):
+    _fields_ = [("capacity", C.c_int), ("n", C.c_int), ("u", c_fp), ("v", c_fp), ("score", c_fp), ("is_corner", C.POINTER(C.c_uint8)),
+                ("angle", c_fp), ("descriptor", C.POINTER(C.c_uint8)), ("n_corners", C.c_int)]
+
+
 # every symbol include/ldso_b200.h declares (tests check the shared object exports all of them)
 SYMBOLS = [
     "ldso_b200_default_settings", "ldso_b200_create", "ldso_b200_destroy", "ldso_b200_last_error", "ldso_b200_set_stream",
     "ldso_b200_synchronize", "ldso_b200_launch_count", "ldso_b200_kernel_times", "ldso_b200_upload_frame", "ldso_b200_make_images",
-    "ldso_b200_download_frame_level", "ldso_b200_set_undistort", "ldso_b200_undistort_frame", "ldso_b200_set_window", "ldso_b200_set_frames", "ldso_b200_set_marg_prior",
+    "ldso_b200_download_frame_level", "ldso_b200_set_undistort", "ldso_b200_undistort_frame",
+    "ldso_b200_set_orb_pattern", "ldso_b200_feature_capacity", "ldso_b200_detect_corners", "ldso_b200_set_window", "ldso_b200_set_frames", "ldso_b200_set_marg_prior",
     "ldso_b200_get_marg_prior", "ldso_b200_linearize_all", "ldso_b200_apply_res", "ldso_b200_backup_state",
     "ldso_b200_solve_system", "ldso_b200_get_system", "ldso_b200_do_step", "ldso_b200_marginalize_points", "ldso_b200_marginalize_frame", "ldso_b200_calc_energies", "ldso_b200_accumulate", "ldso_b200_select_activation", "ldso_b200_init_calc_res", "ldso_b200_optimize_begin",
     "ldso_b200_gn_iterations", "ldso_b200_gn_iterations_until", "ldso_b200_get_iterations_run", "ldso_b200_get_until_form",
@@ -111,6 +117,9 @@ def load():
         L.ldso_b200_set_stream.argtypes = [C.c_void_p, C.c_void_p]
         L.ldso_b200_set_undistort.argtypes = [C.c_void_p, C.POINTER(UndistortCalibC)]
         L.ldso_b200_undistort_frame.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_float, c_fp]
+        L.ldso_b200_set_orb_pattern.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
+        L.ldso_b200_feature_capacity.argtypes = [C.c_int, C.c_int, C.c_int]
+        L.ldso_b200_detect_corners.argtypes = [C.c_void_p, C.c_int, C.c_int, c_fp, C.POINTER(FeaturesC)]
         for name in SYMBOLS:
             fn = getattr(L, name)
             if name not in ("ldso_b200_create", "ldso_b200_destroy", "ldso_b200_last_error", "ldso_b200_launch_count",
@@ -129,6 +138,15 @@ def optimize_iteration_budget(nF, max_its=6) -> int:
     r = load().ldso_b200_optimize_iteration_budget(int(nF), int(max_its))
     if r < 0:
         raise Error(f"ldso_b200_optimize_iteration_budget({nF}, {max_its}) failed: {r}")
+    return r
+
+
+def feature_capacity(w, h, n_features) -> int:
+    """ldso_b200_feature_capacity: the most features DetectCorners can return for a w x h image and n_features; raises for a
+    configuration the device refuses (n_features <= 0, gridsize 0, or patches that can leave the image)."""
+    r = load().ldso_b200_feature_capacity(int(w), int(h), int(n_features))
+    if r < 0:
+        raise Error(f"ldso_b200_feature_capacity({w}, {h}, {n_features}) refused: {r}")
     return r
 
 
@@ -256,6 +274,36 @@ class Context:
         self._chk(self.L.ldso_b200_undistort_frame(self.ctx, int(slot), raw.ctypes.data_as(C.c_void_p), raw.itemsize, float(exposure),
                                                    float(factor), C.byref(e)))
         return float(e.value)
+
+    # ---- keyframe corners (FeatureDetector::DetectCorners on the device)
+    def set_orb_pattern(self, pattern):
+        """ldso_b200_set_orb_pattern: LDSO's bit_pattern_31_ (1024 ints, 256 x 4)."""
+        pat = np.ascontiguousarray(pattern, np.int32).reshape(-1)
+        if pat.size != 1024:
+            raise ValueError(f"the ORB pattern has {pat.size} entries, expected 1024")
+        self._chk(self.L.ldso_b200_set_orb_pattern(self.ctx, pat.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def detect_corners(self, slot, n_features, B=None, capacity=None) -> dict:
+        """ldso_b200_detect_corners on the image in `slot`: DetectCorners(n_features) with CalibHessian::B (256 floats, None = identity).
+        Returns a dict of arrays in the reference's order (u, v, score, is_corner, angle, descriptor n x 32) and n_corners. capacity
+        defaults to feature_capacity(w, h, n_features) (at least 1)."""
+        if capacity is None:
+            r = self.L.ldso_b200_feature_capacity(self.w, self.h, int(n_features))
+            capacity = max(int(r), 1)
+        o = dict(u=np.zeros(capacity, np.float32), v=np.zeros(capacity, np.float32), score=np.zeros(capacity, np.float32),
+                 is_corner=np.zeros(capacity, np.uint8), angle=np.zeros(capacity, np.float32),
+                 descriptor=np.zeros((capacity, 32), np.uint8))
+        f = FeaturesC(int(capacity), 0, _f(o["u"]), _f(o["v"]), _f(o["score"]), _b(o["is_corner"]), _f(o["angle"]),
+                      _b(o["descriptor"]), 0)
+        Bc = None
+        if B is not None:
+            Bc = np.ascontiguousarray(B, np.float32).reshape(-1)
+            if Bc.size != 256:
+                raise ValueError(f"B has {Bc.size} entries, expected 256")
+        self._chk(self.L.ldso_b200_detect_corners(self.ctx, int(slot), int(n_features), _f(Bc), C.byref(f)))
+        out = {k: a[:f.n] for k, a in o.items()}
+        out["n_corners"] = int(f.n_corners)
+        return out
 
     # ---- window
     def set_frames(self, Rcw, tcw, state_zero, state, ab_exposure, frame_id, slots, K_scaled, K_zero=None,

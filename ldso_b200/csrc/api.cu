@@ -22,6 +22,7 @@
 #include "gn_loop.cuh"
 #include "finish.cuh"
 #include "undistort.cuh"
+#include "corners.cuh"
 
 static_assert(K1_THREADS / 32 == MAXF, "phase B maps one warp to one target frame");
 
@@ -49,6 +50,13 @@ struct ldso_b200_ctx {
     float *ud_G = nullptr, *ud_vinv = nullptr;
     void *ud_raw = nullptr, *ud_pin = nullptr;
     cudaEvent_t ud_copied = nullptr;       // the staging buffer has been read by the last frame's copy
+    // keyframe corners (detect_corners), sized at creation for the most features any density can give (one per pixel): the ORB
+    // pattern, B, the per-cell scratch, and the output block [n, scoreTH | u | v | score | angle | is_corner | descriptor] with its
+    // pinned read-back copy
+    int *orb_pattern = nullptr;
+    bool have_orb_pattern = false;
+    float *corner_B = nullptr;
+    char *corner_mem = nullptr, *corner_pin = nullptr;
 
     // window
     DevWindow d;
@@ -210,6 +218,28 @@ extern "C" void ldso_b200_default_settings(ldso_b200_settings *s) {
     s->trace_GNIterations = 3;
 }
 
+// detect_corners' device block, sized for one feature per pixel (px = w*h): the output block first (n, scoreTH, then u | v | score |
+// angle | is_corner | descriptor, laid out per call with that call's capacity), then the ORB pattern, B and the per-cell scratch.
+// Every region starts on a 16-byte boundary whatever w*h is.
+struct CornerLayout { size_t out_bytes, pattern, B, keys, cell_count, cell_off, pick_px, cell_max, pick_score, initial, total; };
+static size_t align16(size_t n) { return (n + 15) & ~(size_t) 15; }
+static CornerLayout corner_layout(size_t px) {
+    CornerLayout L;
+    size_t o = 0;
+    L.out_bytes = align16(16 + px * CORNER_FEATURE_BYTES); o = L.out_bytes;
+    L.pattern = o; o = align16(o + 1024 * sizeof(int));
+    L.B = o; o = align16(o + 256 * sizeof(float));
+    L.keys = o; o = align16(o + px * sizeof(unsigned long long));
+    L.cell_count = o; o = align16(o + px * sizeof(int));
+    L.cell_off = o; o = align16(o + px * sizeof(int));
+    L.pick_px = o; o = align16(o + px * sizeof(int));
+    L.cell_max = o; o = align16(o + px * sizeof(float));
+    L.pick_score = o; o = align16(o + px * sizeof(float));
+    L.initial = o; o = align16(o + px);
+    L.total = o;
+    return L;
+}
+
 extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_levels, const ldso_b200_settings *settings) {
     if (w <= 0 || h <= 0 || pyr_levels < 1 || pyr_levels > MAXLVL) return nullptr;
     int ndev = 0;
@@ -263,6 +293,13 @@ extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_lev
     c->sb.dg = p; p += MAXN; c->sb.bFg = p; p += MAXN;
     ok = cudaMallocHost(&c->sol_host, sizeof(double) * (nn + 3 * MAXN)) == cudaSuccess;      // [lastHS | lastbS | lastX | scalars]
     if (!ok) { fprintf(stderr, "ldso_b200: pinned allocation failed\n"); delete c; return nullptr; }
+    {
+        const CornerLayout L = corner_layout((size_t) w * h);
+        ok = cudaMalloc(&c->corner_mem, L.total) == cudaSuccess && cudaMallocHost(&c->corner_pin, L.out_bytes) == cudaSuccess;
+        if (!ok) { fprintf(stderr, "ldso_b200: corner scratch allocation failed\n"); delete c; return nullptr; }
+        c->orb_pattern = (int *) (c->corner_mem + L.pattern);
+        c->corner_B = (float *) (c->corner_mem + L.B);
+    }
     c->ktime = getenv("LDSO_B200_KTIME") != nullptr;
     c->use_graph = !c->ktime && getenv("LDSO_B200_NO_GRAPH") == nullptr;
     c->use_pdl = getenv("LDSO_B200_NO_PDL") == nullptr;
@@ -318,6 +355,8 @@ extern "C" void ldso_b200_destroy(ldso_b200_ctx *c) {
     if (c->cd_in) cudaFree(c->cd_in);
     if (c->scratch) cudaFree(c->scratch);
     free_undistort(c);
+    if (c->corner_mem) cudaFree(c->corner_mem);
+    if (c->corner_pin) cudaFreeHost(c->corner_pin);
     if (c->ws_dev) cudaFree(c->ws_dev);
     if (c->ws_host) cudaFreeHost(c->ws_host);
     if (c->sol_host) cudaFreeHost(c->sol_host);
@@ -498,6 +537,133 @@ extern "C" int ldso_b200_undistort_frame(ldso_b200_ctx *c, int slot, const void 
     LAUNCH_CHECK(c);
     RET_IF(pyramid_from_scratch(c, slot));
     if (exposure_time_out) *exposure_time_out = c->ud.use_exposure ? exposure : 1.f;
+    return LDSO_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- keyframe corners (corners.cuh)
+namespace {
+struct CornerGrid { int gs, gridX, gridY, skip, ncx, ncy, kcap; float nfeatInGrid; };
+}
+// DetectCorners' grid (FeatureDetector.cc:37-42); false for nFeatures <= 0, gridsize 0, or a grid whose angle / descriptor footprints
+// (+-15 pixels around every pixel of a processed cell: IC_Angle's circle; the descriptor's rotated pattern reaches at most 13) can
+// leave the image, where the reference reads outside its buffer
+static bool corner_grid(int w, int h, int nFeatures, CornerGrid &g) {
+    if (w <= 0 || h <= 0 || nFeatures <= 0) return false;
+    g.gs = int(sqrtf((float) (w * h / nFeatures)) + 0.5);
+    if (g.gs <= 0) return false;
+    g.gridX = w / g.gs + 1;
+    g.gridY = h / g.gs + 1;
+    g.nfeatInGrid = float(nFeatures) / (w * h) * (g.gs * g.gs);
+    g.skip = CORNER_HALF_PATCH * 2 / g.gs + 1;
+    g.ncx = std::max(0, g.gridX - 2 * g.skip);
+    g.ncy = std::max(0, g.gridY - 2 * g.skip);
+    int k = 0;                        // the reference stops after the pick that makes `picked > nfeatInGrid`
+    while (!((float) k > g.nfeatInGrid)) k++;
+    g.kcap = std::min(k, g.gs * g.gs);
+    if (g.ncx > 0 && g.ncy > 0) {
+        const int x0 = g.skip * g.gs, x1 = (g.gridX - g.skip) * g.gs - 1, y0 = g.skip * g.gs, y1 = (g.gridY - g.skip) * g.gs - 1;
+        if (x0 - CORNER_HALF_PATCH < 0 || x1 + CORNER_HALF_PATCH > w - 1 || y0 - CORNER_HALF_PATCH < 0 || y1 + CORNER_HALF_PATCH > h - 1)
+            return false;
+    }
+    return true;
+}
+
+extern "C" int ldso_b200_feature_capacity(int w, int h, int nFeatures) {
+    CornerGrid g;
+    if (!corner_grid(w, h, nFeatures, g)) return LDSO_B200_ERR_ARG;
+    return g.ncx * g.ncy * g.kcap;
+}
+
+extern "C" int ldso_b200_set_orb_pattern(ldso_b200_ctx *c, const int32_t *pattern) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    if (!pattern) return c->fail(LDSO_B200_ERR_ARG, "set_orb_pattern: pattern is NULL");
+    cudaSetDevice(c->device);
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    CUDA_CHECK_RET(c, cudaMemcpy(c->orb_pattern, pattern, sizeof(int32_t) * 1024, cudaMemcpyHostToDevice));
+    c->have_orb_pattern = true;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeatures, const float *B, ldso_b200_features *out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    if (!c->have_orb_pattern) return c->fail(LDSO_B200_ERR_STATE, "detect_corners: call set_orb_pattern first");
+    if (slot < 0 || slot >= NSLOTS || !c->img[slot][0]) return c->fail(LDSO_B200_ERR_ARG, "detect_corners: image slot out of range or never filled");
+    if (!out || !out->u || !out->v || !out->score || !out->is_corner || !out->angle || !out->descriptor)
+        return c->fail(LDSO_B200_ERR_ARG, "detect_corners: missing output array");
+    CornerGrid g;
+    if (!corner_grid(c->w, c->h, nFeatures, g))
+        return c->fail(LDSO_B200_ERR_ARG, "detect_corners: nFeatures must be positive and give a grid whose patches stay inside the image");
+    const int cap = g.ncx * g.ncy * g.kcap;
+    if (out->capacity < cap) return c->fail(LDSO_B200_ERR_ARG, "detect_corners: capacity below ldso_b200_feature_capacity(w, h, nFeatures)");
+    cudaSetDevice(c->device);
+    const size_t px = (size_t) c->w * c->h;
+    CornerArgs a;
+    a.img = c->img[slot][0];
+    a.B = nullptr;
+    if (B) {
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(c->corner_B, B, sizeof(float) * 256, cudaMemcpyHostToDevice, c->stream));
+        a.B = c->corner_B;
+    }
+    a.pattern = c->orb_pattern;
+    a.w = c->w; a.h = c->h;
+    a.gs = g.gs; a.skip = g.skip; a.ncx = g.ncx; a.ncy = g.ncy; a.kcap = g.kcap; a.nfeatInGrid = g.nfeatInGrid;
+    {   // FeatureDetector's constructor (:10-28): umax with cvFloor / cvCeil / cvRound (round half to even)
+        int v, v0, vmax = (int) floor(CORNER_HALF_PATCH * sqrtf(2.f) / 2 + 1), vmin = (int) ceil(CORNER_HALF_PATCH * sqrtf(2.f) / 2);
+        const double hp2 = CORNER_HALF_PATCH * CORNER_HALF_PATCH;
+        for (v = 0; v <= vmax; ++v) a.umax[v] = (int) lrint(sqrt(hp2 - v * v));
+        for (v = CORNER_HALF_PATCH, v0 = 0; v >= vmin; --v) {
+            while (a.umax[v0] == a.umax[v0 + 1]) ++v0;
+            a.umax[v] = v0;
+            ++v0;
+        }
+    }
+    const CornerLayout L = corner_layout(px);
+    char *m = c->corner_mem;
+    a.keys = (unsigned long long *) (m + L.keys);
+    a.cell_count = (int *) (m + L.cell_count);
+    a.cell_off = (int *) (m + L.cell_off);
+    a.pick_px = (int *) (m + L.pick_px);
+    a.cell_max = (float *) (m + L.cell_max);
+    a.pick_score = (float *) (m + L.pick_score);
+    a.initial = (uint8_t *) (m + L.initial);
+    // the output block at the start, laid out with this call's capacity so that one copy brings it back
+    char *o = m;
+    a.hdr = (int *) o;
+    a.cap = cap;
+    a.u = (float *) (o + 16); a.v = a.u + cap; a.score = a.v + cap; a.angle = a.score + cap;
+    a.is_corner = (uint8_t *) (a.angle + cap); a.desc = a.is_corner + cap;
+    const size_t out_bytes = 16 + (size_t) cap * CORNER_FEATURE_BYTES;
+    const int ncell = g.ncx * g.ncy;
+    if (ncell == 0) {
+        CUDA_CHECK_RET(c, cudaMemsetAsync(a.hdr, 0, 16, c->stream));
+    } else {
+        k_corner_cells<<<ncell, CORNER_THREADS, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+        k_corner_scan<<<1, 1024, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+        const int npick = ncell * g.kcap;
+        k_corner_emit<<<(npick + 255) / 256, 256, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+        k_corner_describe<<<(npick + 127) / 128, 128, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+    }
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->corner_pin, o, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    const char *q = c->corner_pin;
+    int n;
+    memcpy(&n, q, sizeof(int));
+    const float *hu = (const float *) (q + 16), *hv = hu + cap, *hs = hv + cap, *ha = hs + cap;
+    const uint8_t *hc = (const uint8_t *) (ha + cap), *hd = hc + cap;
+    memcpy(out->u, hu, sizeof(float) * n);
+    memcpy(out->v, hv, sizeof(float) * n);
+    memcpy(out->score, hs, sizeof(float) * n);
+    memcpy(out->angle, ha, sizeof(float) * n);
+    memcpy(out->is_corner, hc, n);
+    memcpy(out->descriptor, hd, (size_t) 32 * n);
+    int nc = 0;
+    for (int i = 0; i < n; i++) nc += hc[i] != 0;
+    out->n = n;
+    out->n_corners = nc;
     return LDSO_B200_OK;
 }
 
