@@ -458,6 +458,74 @@ int ldso_b200_select_activation(ldso_b200_ctx *ctx, int newest_frame, float curr
                                 const int32_t *lastTraceStatus, const float *lastTracePixelInterval, const float *quality,
                                 const float *my_type, const uint8_t *frame_flagged, uint8_t *action, float *dist_map);
 
+/* ---- the immature-point store: every keyframe's ImmaturePoints resident on the context ------------------
+ * One segment per image slot holds the candidates of the keyframe seeded from that slot, in feature-index order: the fields of
+ * ImmaturePoint (ImmaturePoint.h:103-121) and a live flag (feat->status == IMMATURE && feat->ip). A segment belongs to its slot
+ * key, not to the pixels in it: seeding reads the slot's image, tracing reads only the traced frame's image, activation reads the
+ * window's images through set_frames, and uploading into a slot leaves its segment alone. Every segment has the same capacity: the
+ * largest of ldso_b200_feature_capacity(w, h, nFeatures) over the densities make_new_traces was called with and the counts
+ * immature_seed was given. The store is allocated on first use and grows when a call needs more; growing keeps every segment's
+ * entries, live or released. make_new_traces with a density whose capacity exceeds the store's while any entry is live returns
+ * LDSO_B200_ERR_STATE (LDSO's density is a fixed setting; the per-keyframe path never grows the store). Single, unsharded contexts
+ * only: on a sharded context every store entry point returns LDSO_B200_ERR_STATE. */
+#define LDSO_B200_FEATURE_VALID 1      /* Feature::FeatureStatus (include/Feature.h:38-42) */
+#define LDSO_B200_FEATURE_OUTLIER 2
+/* FullSystem::makeNewTraces with setting_pointSelection == 1 (FullSystem.cc:1274-1283): ldso_b200_detect_corners on `slot`, then the
+ * ImmaturePoint constructor with type 1 for every feature on the device (the features' coordinates never leave it), with the fresh
+ * trace state (idepth_min 0, idepth_max NaN, quality 10000, UNINITIALIZED). Replaces the slot's segment; every feature is kept,
+ * including those whose energyTH is not finite. *out is what detect_corners returns, with its errors; a density whose grid has no
+ * cells gives no features and an empty segment, as detect_corners gives none. */
+int ldso_b200_make_new_traces(ldso_b200_ctx *ctx, int slot, int nFeatures, const float *B, ldso_b200_features *out);
+/* The ImmaturePoint constructor for n coordinates the caller already has (my_type may be NULL: type 1). Replaces the slot's segment.
+ * LDSO_B200_ERR_ARG for a slot out of range or never filled, or a coordinate whose pattern leaves the image (2 <= u < w-3,
+ * 2 <= v < h-3); a refused call leaves the segment as it was. Seeding any count succeeds whatever is live: the store grows. */
+int ldso_b200_immature_seed(ldso_b200_ctx *ctx, int slot, int n, const float *u, const float *v, const float *my_type);
+/* One FullSystem::traceNewCoarse pass (FullSystem.cc:1012-1050) on the frame in image slot new_slot: ImmaturePoint::traceOn of every
+ * live entry of the segments host_slots[0..n_hosts-1], in place, with host j's KRKi9[9j..] (row-major), Kt3[3j..] and aff2[2j..]
+ * computed as FullSystem.cc:1027-1032 does; same bits as ldso_b200_trace_immature. counts7 (may be NULL) receives trace_total,
+ * good, oob, out, skip, badcondition, uninitialized; without it the call is asynchronous and copies nothing. An empty segment
+ * contributes nothing; a slot out of range or listed twice is LDSO_B200_ERR_ARG. */
+int ldso_b200_trace_new_coarse(ldso_b200_ctx *ctx, int new_slot, int n_hosts, const int32_t *host_slots, const float *KRKi9, const float *Kt3,
+                               const float *aff2, int32_t counts7[7]);
+/* The entries activate_immature released, in the reference's visiting order; every array holds `capacity` rows. */
+typedef struct ldso_b200_activation_out {
+    int capacity;                   /* rows; at least the live candidates of window frames 0..nF-2 */
+    int n;                          /* out: released candidates */
+    int n_valid;                    /* out: of which VALID */
+    int32_t *frame;                 /* window frame of the candidate's keyframe */
+    int32_t *index;                 /* feature index in that keyframe (position in its segment) */
+    int32_t *status;                /* LDSO_B200_FEATURE_VALID or LDSO_B200_FEATURE_OUTLIER */
+    float *idepth_min, *idepth_max; /* the ImmaturePoint's interval */
+    float *idepth;                  /* optimizeImmaturePoint's idepth for a selected candidate; NaN for one deleted before it */
+    float *color8, *weights8;       /* [capacity*8] */
+    float *energyTH, *my_type;
+    uint8_t *res_state;             /* [capacity*nF]: per window frame, the final ResState of the residual (255 for the host) -
+                                     * every IN residual of a VALID row becomes a PointFrameResidual (:980-1009) */
+} ldso_b200_activation_out;
+/* FullSystem::activatePointsMT after its currentMinActDist update (FullSystem.cc:1075-1188) on the store: window frame f is the
+ * segment of set_frames' image_slot[f]; the candidates are the live entries of frames 0..nF-2 in window order, then feature-index
+ * order. The selection (as ldso_b200_select_activation), optimizeImmaturePoint of the selected ones (as ldso_b200_optimize_immature)
+ * and the reference's bookkeeping run on the device: deleted candidates (action 2) are released as OUTLIER, selected ones as
+ * VALID when the optimisation succeeds and as OUTLIER otherwise, the rest stay live. LDSO_B200_ERR_STATE before set_frames /
+ * set_window; LDSO_B200_ERR_ARG for a NULL frame_flagged or output array, a capacity below the candidate count, or a level-1
+ * image over select_activation's limit. */
+int ldso_b200_activate_immature(ldso_b200_ctx *ctx, float current_min_act_dist, float min_trace_quality, const uint8_t *frame_flagged,
+                                int min_obs, ldso_b200_activation_out *out);
+/* The keyframe leaves the window (FullSystem::marginalizeFrame): every entry of the slot's segment is released. */
+int ldso_b200_immature_release(ldso_b200_ctx *ctx, int slot);
+/* A segment's whole state, released entries included; arrays of `capacity` rows (color8 / weights8 8 per row, gradH4 4, uv2 2). */
+typedef struct ldso_b200_immature_segment {
+    int capacity;                   /* rows the arrays hold: at least the segment's n */
+    int n;                          /* out: entries seeded */
+    float *u, *v, *my_type;
+    float *color8, *weights8, *gradH4, *energyTH;
+    float *idepth_min, *idepth_max, *quality;
+    int32_t *lastTraceStatus;
+    float *lastTraceUV2, *lastTracePixelInterval;
+    uint8_t *live;
+} ldso_b200_immature_segment;
+int ldso_b200_immature_read(ldso_b200_ctx *ctx, int slot, ldso_b200_immature_segment *out);
+
 /* EXPERIMENTAL (written at the end of round 1 against the pinned oracle, compiled, not yet run on hardware):
  * CoarseInitializer::calcResAndGS (src/frontend/CoarseInitializer.cc:181-405) for the n points of pyramid level lvl. Images: slot
  * first_slot = firstFrame, new_slot = newFrame (upload_frame / make_images). (R, t) = refToNew, tlog3 = refToNew.log().head<3>(),

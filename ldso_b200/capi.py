@@ -77,6 +77,21 @@ class FeaturesC(C.Structure):
                 ("angle", c_fp), ("descriptor", C.POINTER(C.c_uint8)), ("n_corners", C.c_int)]
 
 
+class ActivationOutC(C.Structure):
+    _fields_ = [("capacity", C.c_int), ("n", C.c_int), ("n_valid", C.c_int), ("frame", c_ip), ("index", c_ip), ("status", c_ip),
+                ("idepth_min", c_fp), ("idepth_max", c_fp), ("idepth", c_fp), ("color8", c_fp), ("weights8", c_fp), ("energyTH", c_fp),
+                ("my_type", c_fp), ("res_state", c_bp)]
+
+
+class ImmatureSegmentC(C.Structure):
+    _fields_ = [("capacity", C.c_int), ("n", C.c_int), ("u", c_fp), ("v", c_fp), ("my_type", c_fp), ("color8", c_fp), ("weights8", c_fp),
+                ("gradH4", c_fp), ("energyTH", c_fp), ("idepth_min", c_fp), ("idepth_max", c_fp), ("quality", c_fp), ("lastTraceStatus", c_ip),
+                ("lastTraceUV2", c_fp), ("lastTracePixelInterval", c_fp), ("live", c_bp)]
+
+
+FEATURE_VALID, FEATURE_OUTLIER = 1, 2          # LDSO_B200_FEATURE_*
+
+
 # every symbol include/ldso_b200.h declares (tests check the shared object exports all of them)
 SYMBOLS = [
     "ldso_b200_default_settings", "ldso_b200_create", "ldso_b200_destroy", "ldso_b200_last_error", "ldso_b200_set_stream",
@@ -94,6 +109,8 @@ SYMBOLS = [
     "ldso_b200_trace_immature", "ldso_b200_optimize_immature", "ldso_b200_tracker_make_k",
     "ldso_b200_tracker_set_ref_level", "ldso_b200_tracker_make_coarse_depth", "ldso_b200_tracker_get_ref_level",
     "ldso_b200_tracker_set_frames", "ldso_b200_tracker_eval", "ldso_b200_tracker_track", "ldso_b200_tracker_track_batch", "ldso_b200_posegraph_optimize",
+    "ldso_b200_make_new_traces", "ldso_b200_immature_seed", "ldso_b200_trace_new_coarse", "ldso_b200_activate_immature",
+    "ldso_b200_immature_release", "ldso_b200_immature_read",
 ]
 
 _lib = None
@@ -120,6 +137,12 @@ def load():
         L.ldso_b200_set_orb_pattern.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
         L.ldso_b200_feature_capacity.argtypes = [C.c_int, C.c_int, C.c_int]
         L.ldso_b200_detect_corners.argtypes = [C.c_void_p, C.c_int, C.c_int, c_fp, C.POINTER(FeaturesC)]
+        L.ldso_b200_make_new_traces.argtypes = [C.c_void_p, C.c_int, C.c_int, c_fp, C.POINTER(FeaturesC)]
+        L.ldso_b200_immature_seed.argtypes = [C.c_void_p, C.c_int, C.c_int, c_fp, c_fp, c_fp]
+        L.ldso_b200_trace_new_coarse.argtypes = [C.c_void_p, C.c_int, C.c_int, c_ip, c_fp, c_fp, c_fp, c_ip]
+        L.ldso_b200_activate_immature.argtypes = [C.c_void_p, C.c_float, C.c_float, c_bp, C.c_int, C.POINTER(ActivationOutC)]
+        L.ldso_b200_immature_release.argtypes = [C.c_void_p, C.c_int]
+        L.ldso_b200_immature_read.argtypes = [C.c_void_p, C.c_int, C.POINTER(ImmatureSegmentC)]
         for name in SYMBOLS:
             fn = getattr(L, name)
             if name not in ("ldso_b200_create", "ldso_b200_destroy", "ldso_b200_last_error", "ldso_b200_launch_count",
@@ -189,6 +212,7 @@ class Context:
         self.nF = 0
         self.nP = 0
         self.nR = 0
+        self._imm_rows = {}          # entries seeded per store segment (default capacities of the store's read-backs)
 
     def close(self):
         if getattr(self, "ctx", None):
@@ -287,6 +311,9 @@ class Context:
         """ldso_b200_detect_corners on the image in `slot`: DetectCorners(n_features) with CalibHessian::B (256 floats, None = identity).
         Returns a dict of arrays in the reference's order (u, v, score, is_corner, angle, descriptor n x 32) and n_corners. capacity
         defaults to feature_capacity(w, h, n_features) (at least 1)."""
+        return self._features_call(self.L.ldso_b200_detect_corners, slot, n_features, B, capacity)
+
+    def _features_call(self, fn, slot, n_features, B, capacity):
         if capacity is None:
             r = self.L.ldso_b200_feature_capacity(self.w, self.h, int(n_features))
             capacity = max(int(r), 1)
@@ -300,9 +327,79 @@ class Context:
             Bc = np.ascontiguousarray(B, np.float32).reshape(-1)
             if Bc.size != 256:
                 raise ValueError(f"B has {Bc.size} entries, expected 256")
-        self._chk(self.L.ldso_b200_detect_corners(self.ctx, int(slot), int(n_features), _f(Bc), C.byref(f)))
+        self._chk(fn(self.ctx, int(slot), int(n_features), _f(Bc), C.byref(f)))
         out = {k: a[:f.n] for k, a in o.items()}
         out["n_corners"] = int(f.n_corners)
+        return out
+
+    # ---- the immature-point store (one segment per image slot, resident between calls)
+    def make_new_traces(self, slot, n_features, B=None, capacity=None) -> dict:
+        """ldso_b200_make_new_traces: detect_corners on `slot` and the ImmaturePoint constructor (type 1) of every feature into the
+        slot's segment. Returns what detect_corners returns."""
+        out = self._features_call(self.L.ldso_b200_make_new_traces, slot, n_features, B, capacity)
+        self._imm_rows[int(slot)] = len(out["u"])
+        return out
+
+    def immature_seed(self, slot, u, v, my_type=None):
+        """ldso_b200_immature_seed: the slot's segment becomes ImmaturePoints at (u, v) with my_type (None: 1), fresh trace state."""
+        u = np.ascontiguousarray(u, np.float32); v = np.ascontiguousarray(v, np.float32)
+        if u.shape != v.shape or u.ndim != 1:
+            raise ValueError("u and v must be 1-D arrays of one length")
+        t = None if my_type is None else np.ascontiguousarray(np.broadcast_to(np.asarray(my_type, np.float32), u.shape))
+        self._chk(self.L.ldso_b200_immature_seed(self.ctx, int(slot), u.shape[0], _f(u), _f(v), _f(t)))
+        self._imm_rows[int(slot)] = u.shape[0]
+
+    def trace_new_coarse(self, new_slot, host_slots, KRKi, Kt, aff, counts=False):
+        """ldso_b200_trace_new_coarse: traceOn of every live entry of the listed segments on the frame in new_slot, with each host's
+        KRKi (nH,3,3), Kt (nH,3), aff (nH,2). counts=True returns the seven traceNewCoarse counters (total, good, oob, outlier,
+        skipped, badcondition, uninitialized); otherwise the call is asynchronous and returns None."""
+        hs = np.ascontiguousarray(host_slots, np.int32).reshape(-1)
+        nH = hs.shape[0]
+        K = np.ascontiguousarray(KRKi, np.float32).reshape(nH, 9); t = np.ascontiguousarray(Kt, np.float32).reshape(nH, 3)
+        a = np.ascontiguousarray(aff, np.float32).reshape(nH, 2)
+        c7 = np.zeros(7, np.int32) if counts else None
+        self._chk(self.L.ldso_b200_trace_new_coarse(self.ctx, int(new_slot), nH, _i(hs), _f(K), _f(t), _f(a), _i(c7)))
+        return c7
+
+    def activate_immature(self, current_min_act_dist, frame_flagged=None, min_trace_quality=3.0, min_obs=1, capacity=None) -> dict:
+        """ldso_b200_activate_immature: activatePointsMT on the store against the device-resident window. Returns the released
+        candidates in visiting order (frame, index, status, idepth_min, idepth_max, idepth, color (n,8), weights (n,8), energyTH,
+        my_type, res_state (n,nF)) and n_valid. capacity defaults to every entry this Context has seeded."""
+        nF = max(self.nF, 1)
+        flagged = np.zeros(nF, np.uint8) if frame_flagged is None else np.ascontiguousarray(frame_flagged, np.uint8)
+        if capacity is None:
+            capacity = max(1, sum(self._imm_rows.values()))
+        cap = int(capacity)
+        o = dict(frame=np.zeros(cap, np.int32), index=np.zeros(cap, np.int32), status=np.zeros(cap, np.int32),
+                 idepth_min=np.zeros(cap, np.float32), idepth_max=np.zeros(cap, np.float32), idepth=np.zeros(cap, np.float32),
+                 color=np.zeros((cap, 8), np.float32), weights=np.zeros((cap, 8), np.float32), energyTH=np.zeros(cap, np.float32),
+                 my_type=np.zeros(cap, np.float32), res_state=np.zeros((cap, nF), np.uint8))
+        s = ActivationOutC(cap, 0, 0, _i(o["frame"]), _i(o["index"]), _i(o["status"]), _f(o["idepth_min"]), _f(o["idepth_max"]),
+                           _f(o["idepth"]), _f(o["color"]), _f(o["weights"]), _f(o["energyTH"]), _f(o["my_type"]), _b(o["res_state"]))
+        self._chk(self.L.ldso_b200_activate_immature(self.ctx, C.c_float(current_min_act_dist), C.c_float(min_trace_quality), _b(flagged),
+                                                     int(min_obs), C.byref(s)))
+        out = {k: a[:s.n] for k, a in o.items()}
+        out["n_valid"] = int(s.n_valid)
+        return out
+
+    def immature_release(self, slot):
+        """ldso_b200_immature_release: every entry of the slot's segment is released (the keyframe left the window)."""
+        self._chk(self.L.ldso_b200_immature_release(self.ctx, int(slot)))
+
+    def immature_read(self, slot, capacity=None) -> dict:
+        """ldso_b200_immature_read: the slot's segment (released entries included) as arrays u, v, my_type, color (n,8), weights (n,8),
+        gradH (n,4), energyTH, idepth_min, idepth_max, quality, status, uv (n,2), interval and live (bool)."""
+        cap = max(1, int(capacity if capacity is not None else self._imm_rows.get(int(slot), 0)))
+        o = dict(u=np.zeros(cap, np.float32), v=np.zeros(cap, np.float32), my_type=np.zeros(cap, np.float32), color=np.zeros((cap, 8), np.float32),
+                 weights=np.zeros((cap, 8), np.float32), gradH=np.zeros((cap, 4), np.float32), energyTH=np.zeros(cap, np.float32),
+                 idepth_min=np.zeros(cap, np.float32), idepth_max=np.zeros(cap, np.float32), quality=np.zeros(cap, np.float32),
+                 status=np.zeros(cap, np.int32), uv=np.zeros((cap, 2), np.float32), interval=np.zeros(cap, np.float32), live=np.zeros(cap, np.uint8))
+        s = ImmatureSegmentC(cap, 0, _f(o["u"]), _f(o["v"]), _f(o["my_type"]), _f(o["color"]), _f(o["weights"]), _f(o["gradH"]),
+                             _f(o["energyTH"]), _f(o["idepth_min"]), _f(o["idepth_max"]), _f(o["quality"]), _i(o["status"]), _f(o["uv"]),
+                             _f(o["interval"]), _b(o["live"]))
+        self._chk(self.L.ldso_b200_immature_read(self.ctx, int(slot), C.byref(s)))
+        out = {k: a[:s.n] for k, a in o.items()}
+        out["live"] = out["live"].astype(bool)
         return out
 
     # ---- window

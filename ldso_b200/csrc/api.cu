@@ -18,6 +18,7 @@
 #include "ba_k3.cuh"
 #include "tracker_kernels.cuh"
 #include "trace_types.h"
+#include "immature_store.h"
 #include "posegraph.cuh"
 #include "gn_loop.cuh"
 #include "finish.cuh"
@@ -27,6 +28,7 @@
 static_assert(K1_THREADS / 32 == MAXF, "phase B maps one warp to one target frame");
 
 #define NSLOTS (2 * MAXF)
+static_assert(NSLOTS == IMM_NSEG, "one immature-point segment per image slot");
 
 struct ldso_b200_ctx {
     int device = 0, w = 0, h = 0, levels = 0;
@@ -122,6 +124,12 @@ struct ldso_b200_ctx {
     size_t k1_smem = 0;
     char *trace_buf = nullptr;       // device scratch of immature_init / trace_immature
     size_t trace_cap = 0;
+    // immature-point store (immature_store.h): the segments (imm_cap entries each), activate_immature's scratch and the pinned
+    // read-back block, allocated together on first use; per slot the entries seeded and how many of them are still live
+    float *imm_store = nullptr;
+    char *imm_scratch = nullptr, *imm_pin = nullptr;
+    int imm_cap = 0;
+    int imm_n[NSLOTS] = {}, imm_live[NSLOTS] = {};
     bool multi = false;
     // peer-memory exchange (k2r_peer_allreduce): this rank's exported inbox, the peers' mapped inboxes, and the local
     // epoch / completion / error words
@@ -362,6 +370,9 @@ extern "C" void ldso_b200_destroy(ldso_b200_ctx *c) {
     if (c->sol_host) cudaFreeHost(c->sol_host);
     if (c->actsel_pin) cudaFreeHost(c->actsel_pin);
     if (c->trace_buf) cudaFree(c->trace_buf);
+    if (c->imm_store) cudaFree(c->imm_store);
+    if (c->imm_scratch) cudaFree(c->imm_scratch);
+    if (c->imm_pin) cudaFreeHost(c->imm_pin);
     for (int r = 0; r < K2R_MAX_PEERS; r++) if (c->peer_opened[r]) cudaIpcCloseMemHandle(c->peer_opened[r]);
     if (c->peer_local) cudaFree(c->peer_local);
     if (c->peer_words) cudaFree(c->peer_words);
@@ -584,8 +595,9 @@ extern "C" int ldso_b200_set_orb_pattern(ldso_b200_ctx *c, const int32_t *patter
     return LDSO_B200_OK;
 }
 
-extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeatures, const float *B, ldso_b200_features *out) {
-    if (!c) return LDSO_B200_ERR_ARG;
+// detect_corners' checks and launches on the context's stream; corners_read brings the output block back into *out. Between the two
+// the features are on the device: a.hdr[0] = n, a.u / a.v = their coordinates.
+static int corners_launch(ldso_b200_ctx *c, int slot, int nFeatures, const float *B, const ldso_b200_features *out, CornerArgs &a) {
     if (!c->have_orb_pattern) return c->fail(LDSO_B200_ERR_STATE, "detect_corners: call set_orb_pattern first");
     if (slot < 0 || slot >= NSLOTS || !c->img[slot][0]) return c->fail(LDSO_B200_ERR_ARG, "detect_corners: image slot out of range or never filled");
     if (!out || !out->u || !out->v || !out->score || !out->is_corner || !out->angle || !out->descriptor)
@@ -597,7 +609,6 @@ extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeature
     if (out->capacity < cap) return c->fail(LDSO_B200_ERR_ARG, "detect_corners: capacity below ldso_b200_feature_capacity(w, h, nFeatures)");
     cudaSetDevice(c->device);
     const size_t px = (size_t) c->w * c->h;
-    CornerArgs a;
     a.img = c->img[slot][0];
     a.B = nullptr;
     if (B) {
@@ -632,7 +643,6 @@ extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeature
     a.cap = cap;
     a.u = (float *) (o + 16); a.v = a.u + cap; a.score = a.v + cap; a.angle = a.score + cap;
     a.is_corner = (uint8_t *) (a.angle + cap); a.desc = a.is_corner + cap;
-    const size_t out_bytes = 16 + (size_t) cap * CORNER_FEATURE_BYTES;
     const int ncell = g.ncx * g.ncy;
     if (ncell == 0) {
         CUDA_CHECK_RET(c, cudaMemsetAsync(a.hdr, 0, 16, c->stream));
@@ -647,7 +657,13 @@ extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeature
         k_corner_describe<<<(npick + 127) / 128, 128, 0, c->stream>>>(a);
         LAUNCH_CHECK(c);
     }
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->corner_pin, o, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    return LDSO_B200_OK;
+}
+
+static int corners_read(ldso_b200_ctx *c, const CornerArgs &a, ldso_b200_features *out) {
+    const int cap = a.cap;
+    const size_t out_bytes = 16 + (size_t) cap * CORNER_FEATURE_BYTES;
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->corner_pin, a.hdr, out_bytes, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     const char *q = c->corner_pin;
     int n;
@@ -665,6 +681,13 @@ extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeature
     out->n = n;
     out->n_corners = nc;
     return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeatures, const float *B, ldso_b200_features *out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    CornerArgs a;
+    RET_IF(corners_launch(c, slot, nFeatures, B, out, a));
+    return corners_read(c, a, out);
 }
 
 extern "C" int ldso_b200_download_frame_level(ldso_b200_ctx *c, int slot, int lvl, float *out) {
@@ -1562,6 +1585,280 @@ extern "C" int ldso_b200_select_activation(ldso_b200_ctx *c, int newest_frame, f
     if (A.dbg) fprintf(stderr, "[ldso_b200 actsel] cycles: map+seeds+grow %lld, candidate terms %lld, sequential pass %lld\n", stamps[1] - stamps[0],
                        stamps[2] - stamps[1], stamps[3] - stamps[2]);
     if (dist_map) for (size_t i = 0; i < cells; i++) dist_map[i] = c->h_scratch_bytes[i] == 255 ? 1000.f : (float) c->h_scratch_bytes[i];   // fwdWarpedIDDistFinal's values
+    return LDSO_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- immature-point store
+// activate_immature's device scratch (sized for every candidate of a full window: (MAXF-1) segments) and the pinned block, whose
+// first 64 bytes hold the header, traceNewCoarse's counters and the frame flags, and the rest a segment or the released records
+// scratch: 38 words per candidate (gathered, k_activation_select's terms, selected, LM results), res_state and action bytes, the two
+// BFS frontiers, the distance map, 64 bytes of flags / header / counters, the released records
+struct ImmLayout { size_t maxc, cells, map_bytes, bytes, front, map, small, rec, scratch, pin; };
+static ImmLayout imm_layout(const ldso_b200_ctx *c, int cap) {
+    ImmLayout L;
+    L.maxc = (size_t) (MAXF - 1) * cap;
+    L.cells = (size_t) (c->w >> 1) * (c->h >> 1);
+    L.map_bytes = (L.cells + 3) & ~(size_t) 3;
+    L.bytes = align16(L.maxc * 4 * 38);
+    L.front = L.bytes + align16(L.maxc * (MAXF + 1));
+    L.map = L.front + align16(8 * L.cells);
+    L.small = L.map + align16(L.map_bytes);
+    L.rec = L.small + 64;
+    L.scratch = L.rec + L.maxc * sizeof(ImmRecord);
+    L.pin = 64 + std::max((size_t) IMM_SEG_WORDS * 4 * cap, L.maxc * sizeof(ImmRecord));
+    return L;
+}
+static cudaError_t imm_copy_segment(const ImmSeg &d, const ImmSeg &s, size_t n, cudaStream_t st) {
+    const struct { void *dst; const void *src; size_t words; } f[] = {
+        {d.u, s.u, 1}, {d.v, s.v, 1}, {d.my_type, s.my_type, 1}, {d.color8, s.color8, 8}, {d.weights8, s.weights8, 8}, {d.gradH4, s.gradH4, 4},
+        {d.energyTH, s.energyTH, 1}, {d.idmin, s.idmin, 1}, {d.idmax, s.idmax, 1}, {d.quality, s.quality, 1}, {d.status, s.status, 1},
+        {d.uv2, s.uv2, 2}, {d.interval, s.interval, 1}, {d.live, s.live, 1}};
+    size_t words = 0;
+    for (const auto &x : f) words += x.words;
+    if (words != IMM_SEG_WORDS) return cudaErrorInvalidValue;       // a field of imm_seg missing here
+    for (const auto &x : f) {
+        const cudaError_t e = cudaMemcpyAsync(x.dst, x.src, 4 * x.words * n, cudaMemcpyDeviceToDevice, st);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+// grows the store to at least cap entries per segment; every segment keeps its entries (live or released), copied to the new stride
+static int imm_reserve(ldso_b200_ctx *c, int cap) {
+    if (cap <= c->imm_cap) return LDSO_B200_OK;
+    const ImmLayout L = imm_layout(c, cap);
+    float *store = nullptr;
+    char *scratch = nullptr, *pin = nullptr;
+    cudaError_t e = cudaMalloc(&store, sizeof(float) * IMM_SEG_WORDS * (size_t) cap * NSLOTS);
+    if (e == cudaSuccess) e = cudaMalloc(&scratch, L.scratch);
+    if (e == cudaSuccess) e = cudaMallocHost(&pin, L.pin);
+    for (int s = 0; s < NSLOTS && e == cudaSuccess; s++)
+        if (c->imm_n[s] > 0) e = imm_copy_segment(imm_seg(store, cap, s), imm_seg(c->imm_store, c->imm_cap, s), (size_t) c->imm_n[s], c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) {
+        if (store) cudaFree(store);
+        if (scratch) cudaFree(scratch);
+        if (pin) cudaFreeHost(pin);
+        return c->fail_cuda(e, "immature store growth", __FILE__, __LINE__);
+    }
+    if (c->imm_store) cudaFree(c->imm_store);
+    if (c->imm_scratch) cudaFree(c->imm_scratch);
+    if (c->imm_pin) cudaFreeHost(c->imm_pin);
+    c->imm_store = store; c->imm_scratch = scratch; c->imm_pin = pin; c->imm_cap = cap;
+    return LDSO_B200_OK;
+}
+#define IMM_SINGLE(c, what) do { if ((c)->multi) return (c)->fail(LDSO_B200_ERR_STATE, what " runs on a single, unsharded context"); } while (0)
+
+extern "C" int ldso_b200_make_new_traces(ldso_b200_ctx *c, int slot, int nFeatures, const float *B, ldso_b200_features *out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    IMM_SINGLE(c, "make_new_traces");
+    CornerGrid g;
+    if (!corner_grid(c->w, c->h, nFeatures, g))
+        return c->fail(LDSO_B200_ERR_ARG, "make_new_traces: nFeatures must be positive and give a grid whose patches stay inside the image");
+    CornerArgs a;
+    RET_IF(corners_launch(c, slot, nFeatures, B, out, a));
+    const int need = std::max(1, g.ncx * g.ncy * g.kcap);
+    if (need > c->imm_cap)          // the density fixes the store's capacity: it may change only while nothing is live
+        for (int s = 0; s < NSLOTS; s++)
+            if (c->imm_live[s]) return c->fail(LDSO_B200_ERR_STATE, "make_new_traces: a density with a larger capacity while entries are live");
+    RET_IF(imm_reserve(c, need));
+    c->imm_n[slot] = c->imm_live[slot] = 0;
+    if (a.cap > 0) {                // a grid without cells: detect_corners returns no features, and the segment stays empty
+        launch_store_seed(a.hdr, a.cap, a.u, a.v, nullptr, c->img[slot][0], c->w, trace_settings(c), c->imm_store, c->imm_cap, slot, c->stream);
+        LAUNCH_CHECK(c);
+    }
+    RET_IF(corners_read(c, a, out));
+    c->imm_n[slot] = c->imm_live[slot] = out->n;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_immature_seed(ldso_b200_ctx *c, int slot, int n, const float *u, const float *v, const float *my_type) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    IMM_SINGLE(c, "immature_seed");
+    if (slot < 0 || slot >= NSLOTS || !c->img[slot][0]) return c->fail(LDSO_B200_ERR_ARG, "immature_seed: image slot out of range or never filled");
+    if (n < 0 || (n > 0 && (!u || !v))) return c->fail(LDSO_B200_ERR_ARG, "immature_seed: negative count or missing coordinates");
+    for (int i = 0; i < n; i++)
+        if (!(u[i] >= 2 && u[i] < c->w - 3 && v[i] >= 2 && v[i] < c->h - 3))
+            return c->fail(LDSO_B200_ERR_ARG, "immature_seed: a candidate's pattern leaves the image");
+    cudaSetDevice(c->device);
+    RET_IF(imm_reserve(c, n));
+    c->imm_live[slot] = 0;
+    c->imm_n[slot] = 0;
+    if (n == 0) return LDSO_B200_OK;
+    const ImmSeg g = imm_seg(c->imm_store, c->imm_cap, slot);
+    float *hp = (float *) (c->imm_pin + 64);
+    const size_t N = (size_t) n;
+    memcpy(hp, u, 4 * N); memcpy(hp + N, v, 4 * N);
+    if (my_type) memcpy(hp + 2 * N, my_type, 4 * N);
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(g.u, hp, 4 * N, cudaMemcpyHostToDevice, c->stream));
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(g.v, hp + N, 4 * N, cudaMemcpyHostToDevice, c->stream));
+    if (my_type) CUDA_CHECK_RET(c, cudaMemcpyAsync(g.my_type, hp + 2 * N, 4 * N, cudaMemcpyHostToDevice, c->stream));
+    launch_store_seed(nullptr, n, g.u, g.v, my_type ? g.my_type : nullptr, c->img[slot][0], c->w, trace_settings(c), c->imm_store, c->imm_cap,
+                      slot, c->stream);
+    LAUNCH_CHECK(c);
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    c->imm_n[slot] = c->imm_live[slot] = n;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_trace_new_coarse(ldso_b200_ctx *c, int new_slot, int n_hosts, const int32_t *host_slots, const float *KRKi9,
+                                          const float *Kt3, const float *aff2, int32_t counts7[7]) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    IMM_SINGLE(c, "trace_new_coarse");
+    if (new_slot < 0 || new_slot >= NSLOTS || !c->img[new_slot][0]) return c->fail(LDSO_B200_ERR_ARG, "trace_new_coarse: image slot of the traced frame not filled");
+    if (n_hosts < 0 || n_hosts > NSLOTS || (n_hosts > 0 && (!host_slots || !KRKi9 || !Kt3 || !aff2)))
+        return c->fail(LDSO_B200_ERR_ARG, "trace_new_coarse: bad host list");
+    StoreTraceArgs P;
+    P.nseg = n_hosts;
+    P.begin[0] = 0;
+    for (int j = 0; j < n_hosts; j++) {
+        const int s = host_slots[j];
+        if (s < 0 || s >= NSLOTS) return c->fail(LDSO_B200_ERR_ARG, "trace_new_coarse: host slot out of range");
+        for (int q = 0; q < j; q++) if (host_slots[q] == s) return c->fail(LDSO_B200_ERR_ARG, "trace_new_coarse: host slot listed twice");
+        P.slot[j] = s;
+        P.begin[j + 1] = P.begin[j] + (c->imm_live[s] ? c->imm_n[s] : 0);
+        memcpy(P.KRKi[j], KRKi9 + 9 * j, sizeof(float) * 9); memcpy(P.Kt[j], Kt3 + 3 * j, sizeof(float) * 3); memcpy(P.aff[j], aff2 + 2 * j, sizeof(float) * 2);
+    }
+    if (counts7) memset(counts7, 0, sizeof(int32_t) * 7);
+    if (P.begin[n_hosts] == 0) return LDSO_B200_OK;
+    cudaSetDevice(c->device);
+    memset(&P.T, 0, sizeof(P.T));
+    P.T.w = c->w; P.T.h = c->h; P.T.img = c->img[new_slot][0]; P.T.S = trace_settings(c);
+    P.store = c->imm_store; P.cap = c->imm_cap;
+    const ImmLayout L = imm_layout(c, c->imm_cap);
+    P.counts = counts7 ? (int *) (c->imm_scratch + L.small + 32) : nullptr;
+    if (P.counts) CUDA_CHECK_RET(c, cudaMemsetAsync(P.counts, 0, sizeof(int) * 7, c->stream));
+    launch_store_trace(P, c->stream);
+    LAUNCH_CHECK(c);
+    if (counts7) {
+        int *hc = (int *) (c->imm_pin + 16);
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(hc, P.counts, sizeof(int) * 7, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+        memcpy(counts7, hc, sizeof(int32_t) * 7);
+    }
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_activate_immature(ldso_b200_ctx *c, float current_min_act_dist, float min_trace_quality, const uint8_t *frame_flagged,
+                                           int min_obs, ldso_b200_activation_out *out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    IMM_SINGLE(c, "activate_immature");
+    if (!c->have_frames || !c->have_window) return c->fail(LDSO_B200_ERR_STATE, "activate_immature needs set_frames and set_window first");
+    if (!frame_flagged) return c->fail(LDSO_B200_ERR_ARG, "frame_flagged must hold one byte per frame");
+    if (!out || !out->frame || !out->index || !out->status || !out->idepth_min || !out->idepth_max || !out->idepth || !out->color8 ||
+        !out->weights8 || !out->energyTH || !out->my_type || !out->res_state) return c->fail(LDSO_B200_ERR_ARG, "activate_immature: missing output array");
+    const int nF = c->nF, w1 = c->w >> 1, h1 = c->h >> 1;
+    const size_t cells = (size_t) w1 * h1, map_bytes = (cells + 3) & ~(size_t) 3;
+    if (map_bytes > 200 * 1024) return c->fail(LDSO_B200_ERR_ARG, "activate_immature: level-1 image larger than 200 KB (one byte per pixel must fit in shared memory)");
+    StoreActArgs P;
+    P.nseg = std::max(nF - 1, 0);
+    P.begin[0] = 0;
+    for (int f = 0; f < nF; f++) {
+        P.slot[f] = c->slots[f];
+        if (f < P.nseg) P.begin[f + 1] = P.begin[f] + (c->imm_live[c->slots[f]] ? c->imm_n[c->slots[f]] : 0);
+    }
+    int ncand = 0;
+    for (int f = 0; f < P.nseg; f++) ncand += c->imm_live[c->slots[f]];
+    if (out->capacity < ncand) return c->fail(LDSO_B200_ERR_ARG, "activate_immature: capacity below the number of live candidates");
+    out->n = 0; out->n_valid = 0;
+    if (ncand == 0) return LDSO_B200_OK;
+    cudaSetDevice(c->device);
+    RET_IF(build_derived(c));
+    const ImmLayout L = imm_layout(c, c->imm_cap);
+    const size_t M = L.maxc;
+    P.store = c->imm_store; P.cap = c->imm_cap; P.n = ncand; P.nF = nF; P.ws = c->ws_dev;
+    float *f32 = (float *) c->imm_scratch;
+    P.c_u = f32; P.c_v = f32 + M; P.c_idmin = f32 + 2 * M; P.c_idmax = f32 + 3 * M; P.c_quality = f32 + 4 * M; P.c_interval = f32 + 5 * M;
+    P.c_type = f32 + 6 * M;
+    P.c_status = (int *) (f32 + 7 * M); P.c_host = (int *) (f32 + 8 * M); P.c_index = (int *) (f32 + 9 * M); P.c_sel = (int *) (f32 + 10 * M);
+    ActSelArgs A;
+    A.pre_idx = (int *) (f32 + 11 * M); A.pre_frac = f32 + 12 * M; A.pre_thresh = f32 + 13 * M;
+    P.s_u = f32 + 14 * M; P.s_v = f32 + 15 * M; P.s_idmin = f32 + 16 * M; P.s_idmax = f32 + 17 * M; P.s_energyTH = f32 + 18 * M;
+    P.s_idepth = f32 + 19 * M; P.s_host = (int *) (f32 + 20 * M); P.s_ok = (int *) (f32 + 21 * M);
+    P.s_color8 = f32 + 22 * M; P.s_weights8 = f32 + 30 * M;
+    P.s_res = (unsigned char *) (c->imm_scratch + L.bytes); P.action = P.s_res + M * MAXF;
+    A.front0 = (int *) (c->imm_scratch + L.front); A.front1 = A.front0 + cells;
+    A.map = (unsigned char *) (c->imm_scratch + L.map);
+    unsigned char *dflag = (unsigned char *) (c->imm_scratch + L.small);
+    P.hdr = (int *) (c->imm_scratch + L.small + 16);
+    P.rec = (ImmRecord *) (c->imm_scratch + L.rec);
+    // candidates, selection, activation LM, bookkeeping
+    launch_store_gather(P, c->stream);
+    LAUNCH_CHECK(c);
+    memcpy(c->imm_pin + 48, frame_flagged, (size_t) nF);
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(dflag, c->imm_pin + 48, (size_t) nF, cudaMemcpyHostToDevice, c->stream));
+    A.ws = c->ws_dev; A.newest = nF - 1; A.w1 = w1; A.h1 = h1;
+    A.nP = c->d.nP; A.pt_host = c->d.pt_host; A.pt_u = c->d.pt_u; A.pt_v = c->d.pt_v; A.pt_idepth = c->d.pt_idepth;
+    A.n = ncand;
+    A.u = P.c_u; A.v = P.c_v; A.idmin = P.c_idmin; A.idmax = P.c_idmax; A.quality = P.c_quality; A.interval = P.c_interval; A.my_type = P.c_type;
+    A.status = P.c_status; A.host = P.c_host; A.flagged = dflag;
+    A.currentMinActDist = current_min_act_dist; A.minTraceQuality = min_trace_quality;
+    A.action = P.action; A.map_bytes = (int) map_bytes; A.use_smem = 1; A.dbg = nullptr;
+    launch_activation_select(A, c->stream);
+    LAUNCH_CHECK(c);
+    launch_store_pick(P, c->stream);
+    LAUNCH_CHECK(c);
+    launch_store_optimize(P, min_obs, c->stream);
+    LAUNCH_CHECK(c);
+    launch_store_apply(P, c->stream);
+    LAUNCH_CHECK(c);
+    int *hh = (int *) c->imm_pin;
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(hh, P.hdr, sizeof(int) * 4, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    const int nrel = hh[1], nvalid = hh[2];
+    const ImmRecord *hr = (const ImmRecord *) (c->imm_pin + 64);
+    if (nrel > 0) {
+        CUDA_CHECK_RET(c, cudaMemcpyAsync((void *) hr, P.rec, sizeof(ImmRecord) * nrel, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    }
+    for (int i = 0; i < nrel; i++) {
+        const ImmRecord &r = hr[i];
+        out->frame[i] = r.frame; out->index[i] = r.index; out->status[i] = r.status;
+        out->idepth_min[i] = r.idepth_min; out->idepth_max[i] = r.idepth_max; out->idepth[i] = r.idepth;
+        out->energyTH[i] = r.energyTH; out->my_type[i] = r.my_type;
+        memcpy(out->color8 + 8 * i, r.color8, sizeof(r.color8)); memcpy(out->weights8 + 8 * i, r.weights8, sizeof(r.weights8));
+        memcpy(out->res_state + (size_t) nF * i, r.res_state, (size_t) nF);
+        c->imm_live[c->slots[r.frame]]--;
+    }
+    out->n = nrel; out->n_valid = nvalid;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_immature_release(ldso_b200_ctx *c, int slot) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    IMM_SINGLE(c, "immature_release");
+    if (slot < 0 || slot >= NSLOTS) return c->fail(LDSO_B200_ERR_ARG, "immature_release: slot out of range");
+    if (c->imm_live[slot]) {
+        cudaSetDevice(c->device);
+        CUDA_CHECK_RET(c, cudaMemsetAsync(imm_seg(c->imm_store, c->imm_cap, slot).live, 0, sizeof(int) * c->imm_n[slot], c->stream));
+    }
+    c->imm_live[slot] = 0;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_immature_read(ldso_b200_ctx *c, int slot, ldso_b200_immature_segment *out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    IMM_SINGLE(c, "immature_read");
+    if (slot < 0 || slot >= NSLOTS) return c->fail(LDSO_B200_ERR_ARG, "immature_read: slot out of range");
+    if (!out) return c->fail(LDSO_B200_ERR_ARG, "immature_read: out is NULL");
+    const int n = c->imm_n[slot];
+    if (out->capacity < n) return c->fail(LDSO_B200_ERR_ARG, "immature_read: capacity below the segment's entry count");
+    if (n > 0 && (!out->u || !out->v || !out->my_type || !out->color8 || !out->weights8 || !out->gradH4 || !out->energyTH || !out->idepth_min ||
+                  !out->idepth_max || !out->quality || !out->lastTraceStatus || !out->lastTraceUV2 || !out->lastTracePixelInterval || !out->live))
+        return c->fail(LDSO_B200_ERR_ARG, "immature_read: missing output array");
+    out->n = n;
+    if (n == 0) return LDSO_B200_OK;
+    cudaSetDevice(c->device);
+    const size_t cap = c->imm_cap, N = n;
+    float *hp = (float *) (c->imm_pin + 64);
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(hp, imm_seg(c->imm_store, c->imm_cap, slot).u, sizeof(float) * IMM_SEG_WORDS * cap, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    const ImmSeg g = imm_seg(hp, c->imm_cap, 0);      // the segment's layout, at the staging copy
+    memcpy(out->u, g.u, 4 * N); memcpy(out->v, g.v, 4 * N); memcpy(out->my_type, g.my_type, 4 * N);
+    memcpy(out->color8, g.color8, 32 * N); memcpy(out->weights8, g.weights8, 32 * N); memcpy(out->gradH4, g.gradH4, 16 * N);
+    memcpy(out->energyTH, g.energyTH, 4 * N); memcpy(out->idepth_min, g.idmin, 4 * N); memcpy(out->idepth_max, g.idmax, 4 * N);
+    memcpy(out->quality, g.quality, 4 * N); memcpy(out->lastTraceStatus, g.status, 4 * N); memcpy(out->lastTraceUV2, g.uv2, 8 * N);
+    memcpy(out->lastTracePixelInterval, g.interval, 4 * N);
+    for (int i = 0; i < n; i++) out->live[i] = g.live[i] != 0;
     return LDSO_B200_OK;
 }
 

@@ -29,11 +29,10 @@ __device__ __forceinline__ float3 trace_tap3(const float4 *img, int w, int h, fl
                        w11 * p11.z + w01 * p01.z + w10 * p10.z + w00 * p00.z);
 }
 
-// ImmaturePoint::ImmaturePoint (:14-38): one thread per candidate on its host keyframe
-__global__ void k_immature_init(int n, const float4 *img, int w, const float *u, const float *v, TraceSettingsDev S, float *color8,
-                                float *weights8, float *gradH4, float *energyTH) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+// ImmaturePoint::ImmaturePoint (:14-38) of candidate i: one thread per candidate on its host keyframe. color8 / weights8 past the first
+// non-finite pattern pixel are left as they are.
+__device__ __forceinline__ void immature_init_one(int i, const float4 *img, int w, const float *u, const float *v, const TraceSettingsDev &S,
+                                                  float *color8, float *weights8, float *gradH4, float *energyTH) {
     float g00 = 0, g01 = 0, g10 = 0, g11 = 0;
     bool bad = false;
     for (int idx = 0; idx < 8 && !bad; idx++) {
@@ -57,20 +56,25 @@ __global__ void k_immature_init(int n, const float4 *img, int w, const float *u,
     energyTH[i] = bad ? NAN : e;
 }
 
+__global__ void k_immature_init(int n, const float4 *img, int w, const float *u, const float *v, TraceSettingsDev S, float *color8,
+                                float *weights8, float *gradH4, float *energyTH) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    immature_init_one(i, img, w, u, v, S, color8, weights8, gradH4, energyTH);
+}
+
 #define KTR_WARPS 8
-__global__ void __launch_bounds__(32 * KTR_WARPS) k_trace_on(TraceArgs A) {
-    __shared__ float s_err[KTR_WARPS][100];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const int i = blockIdx.x * KTR_WARPS + wib;
-    if (i >= A.n) return;
+// ImmaturePoint::traceOn of candidate i (one warp; every lane returns the same status, the candidate's lastTraceStatus afterwards).
+// A's per-candidate arrays are indexed by i; KRKi / Kt / aff are the candidate's host transform; s_err is this warp's 100 floats.
+__device__ __forceinline__ int trace_on_one(const TraceArgs &A, int i, const float *KRKi, const float *Kt, const float *aff, float *s_err) {
+    const int lane = threadIdx.x & 31;
     const unsigned FULL = 0xffffffffu;
     const TraceSettingsDev &S = A.S;
     int st = A.status[i];
-    if (st == IPS_OOB) return;                                                   // :52
+    if (st == IPS_OOB) return st;                                                // :52
     const int w = A.w, h = A.h;
     const float pu = A.u[i], pv = A.v[i];
     float idmin = A.idepth_min[i], idmax = A.idepth_max[i], quality = A.quality[i];
-    const float *KRKi = A.KRKi9 + 9 * A.host[i], *Kt = A.Kt3 + 3 * A.host[i], *aff = A.aff2 + 2 * A.host[i];
     const float maxPixSearch = (w + h) * S.maxPixSearch;
     float uvx = -1.f, uvy = -1.f, interval = 0.f;
     int result = -1;          // >= 0: finished with this status
@@ -157,7 +161,7 @@ __global__ void __launch_bounds__(32 * KTR_WARPS) k_trace_on(TraceArgs A) {
                         const float hw = fabsf(residual) < S.huberTH ? 1 : S.huberTH / fabsf(residual);
                         energy += hw * residual * residual * (2 - hw);
                     }
-                    s_err[wib][si] = energy;
+                    s_err[si] = energy;
                     if (energy < myBestE) { myBestE = energy; myBestU = ptx; myBestV = pty; myBestI = si; }
                 }
                 for (int k = 0; k < 32; k++) { ptx += dx; pty += dy; }
@@ -177,7 +181,7 @@ __global__ void __launch_bounds__(32 * KTR_WARPS) k_trace_on(TraceArgs A) {
             __syncwarp();
             float second = 1e10f;                                                // :220-227
             for (int si = lane; si < numSteps; si += 32)
-                if ((si < bestIdx - S.minTraceTestRadius || si > bestIdx + S.minTraceTestRadius) && s_err[wib][si] < second) second = s_err[wib][si];
+                if ((si < bestIdx - S.minTraceTestRadius || si > bestIdx + S.minTraceTestRadius) && s_err[si] < second) second = s_err[si];
             for (int o = 16; o > 0; o >>= 1) second = fminf(second, __shfl_xor_sync(FULL, second, o));
             const float newQuality = second / bestEnergy;
             if (newQuality < quality || numSteps > 10) quality = newQuality;
@@ -247,6 +251,15 @@ __global__ void __launch_bounds__(32 * KTR_WARPS) k_trace_on(TraceArgs A) {
         A.idepth_min[i] = idmin; A.idepth_max[i] = idmax; A.quality[i] = quality;
         A.uv2[2 * i] = uvx; A.uv2[2 * i + 1] = uvy; A.interval[i] = interval;
     }
+    return result;
+}
+
+__global__ void __launch_bounds__(32 * KTR_WARPS) k_trace_on(TraceArgs A) {
+    __shared__ float s_err[KTR_WARPS][100];
+    const int wib = threadIdx.x >> 5;
+    const int i = blockIdx.x * KTR_WARPS + wib;
+    if (i >= A.n) return;
+    trace_on_one(A, i, A.KRKi9 + 9 * A.host[i], A.Kt3 + 3 * A.host[i], A.aff2 + 2 * A.host[i], s_err[wib]);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -336,13 +349,11 @@ __device__ __forceinline__ void immature_eval(const WinState *ws, int nF, int ho
     }
 }
 
-__global__ void __launch_bounds__(32 * KTR_WARPS) k_optimize_immature(int n, const WinState *ws, const float *u, const float *v, const int *host,
-                                                                      const float *idmin, const float *idmax, const float *color8,
-                                                                      const float *weights8, const float *energyTH, int minObs, int *ok_out,
-                                                                      float *idepth_out, unsigned char *res_state) {
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const int i = blockIdx.x * KTR_WARPS + wib;
-    if (i >= n) return;
+// optimizeImmaturePoint of candidate i (one warp)
+__device__ __forceinline__ void optimize_immature_one(int i, const WinState *ws, const float *u, const float *v, const int *host, const float *idmin,
+                                                      const float *idmax, const float *color8, const float *weights8, const float *energyTH,
+                                                      int minObs, int *ok_out, float *idepth_out, unsigned char *res_state) {
+    const int lane = threadIdx.x & 31;
     const int nF = ws->nF, nres = nF - 1, h = host[i];
     const float setting_minIdepthH_act = 100;          // Setting.cc:25
     const int setting_GNItsOnPointActivation = 3;      // Setting.cc:47
@@ -396,6 +407,15 @@ __global__ void __launch_bounds__(32 * KTR_WARPS) k_optimize_immature(int n, con
 #pragma unroll
         for (int r = 0; r < MAXF - 1; r++) if (r < nres) res_state[(size_t) i * nF + ((r < h) ? r : r + 1)] = (unsigned char) st[r];
     }
+}
+
+__global__ void __launch_bounds__(32 * KTR_WARPS) k_optimize_immature(int n, const WinState *ws, const float *u, const float *v, const int *host,
+                                                                      const float *idmin, const float *idmax, const float *color8,
+                                                                      const float *weights8, const float *energyTH, int minObs, int *ok_out,
+                                                                      float *idepth_out, unsigned char *res_state) {
+    const int i = blockIdx.x * KTR_WARPS + (threadIdx.x >> 5);
+    if (i >= n) return;
+    optimize_immature_one(i, ws, u, v, host, idmin, idmax, color8, weights8, energyTH, minObs, ok_out, idepth_out, res_state);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
