@@ -157,6 +157,41 @@ int ldso_b200_feature_capacity(int w, int h, int nFeatures);
  * ImmaturePoints come from ldso_b200_immature_init on the same slot. */
 int ldso_b200_detect_corners(ldso_b200_ctx *ctx, int slot, int nFeatures, const float *B, ldso_b200_features *out);
 
+/* ---- keyframe candidate pixels: DSO's PixelSelector::makeMaps on the device -------------------------------
+ * LDSO's setting_pointSelection == 0 (FullSystem.cc:1284-1304) and the monocular initializer's level-0 selection
+ * (CoarseInitializer::setFirst, CoarseInitializer.cc:552-562). makeHists, select and makeMaps (src/frontend/PixelSelector2.cc) run on
+ * levels 0-2 of a resident slot, bit for bit, with two rules where the reference reads memory it never wrote: thsSmoothed entries
+ * at or past (w/32)*(h/32) read 0, and absSquaredGrad is 0 on rows 0 and h_l-1 of every level (DESIGN.md "Pixel selection"). */
+typedef struct ldso_b200_pixsel_params {
+    float density;                  /* numWant: setting_desiredImmatureDensity (1500), or densities[0]*w*h for the initializer */
+    int recursions_left;            /* makeMaps' recursionsLeft (1) */
+    float th_factor;                /* thFactor (1; the initializer passes 2) */
+    float minGradHistCut;           /* setting_minGradHistCut (0.5) */
+    float minGradHistAdd;           /* setting_minGradHistAdd (7) */
+    float gradDownweightPerLevel;   /* setting_gradDownweightPerLevel (0.75) */
+    int selectDirectionDistribution;/* setting_selectDirectionDistribution (1) */
+} ldso_b200_pixsel_params;
+/* makeMaps' selection map as pixels in raster order; x / y / type hold `capacity` rows. */
+typedef struct ldso_b200_pixels {
+    int capacity;                   /* rows: at least n (w*h always suffices) */
+    int n;                          /* out: makeMaps' return value (numHaveSub): the selected pixels */
+    int n2, n3, n4;                 /* out: select()'s counts of the final pass (before the subsampling) */
+    int32_t *x, *y;
+    uint8_t *type;                  /* PixelSelectorStatus: 1, 2 or 4 */
+    uint8_t *map;                   /* optional (may be NULL): the w*h map, 0 where nothing is selected */
+} ldso_b200_pixels;
+/* PixelSelector::makeMaps(fh, map_out, params->density, params->recursions_left, false, params->th_factor) on the pyramid in `slot`,
+ * with *current_potential the selector's currentPotential: read, and written back as makeMaps leaves it. B is CalibHessian::B (256
+ * floats; NULL = identity), applied as makeImages' gamma weight (setting_gammaWeightsPixelSelect = 1). The histogram is made once per
+ * call; each recursion costs one read-back of the pass's counts. randomPattern is glibc's rand() sequence after srand(3141592),
+ * generated without touching the caller's rand() state. LDSO_B200_ERR_ARG for a context with fewer than 3 pyramid levels, a slot out
+ * of range or never filled, NULL params / current_potential / out / output arrays, density <= 0, *current_potential < 1, or a
+ * capacity below n (nothing is written back then). */
+int ldso_b200_select_pixels(ldso_b200_ctx *ctx, int slot, const ldso_b200_pixsel_params *params, const float *B, int *current_potential,
+                            ldso_b200_pixels *out);
+/* The first n bytes of the selector's randomPattern (PixelSelector2.cc:11-13) as ldso_b200_select_pixels generates them. */
+int ldso_b200_pixsel_pattern(int n, uint8_t *out);
+
 /* ---- the optimisation window ---------------------------------------------------------------------------
  * Flattened EnergyFunctional::allPoints (EnergyFunctional.cc:385-401, points ordered by host keyframe as
  * makeIDX produces them) with each point's PointHessian::residuals list (CSR). */
@@ -476,6 +511,20 @@ int ldso_b200_select_activation(ldso_b200_ctx *ctx, int newest_frame, float curr
  * including those whose energyTH is not finite. *out is what detect_corners returns, with its errors; a density whose grid has no
  * cells gives no features and an empty segment, as detect_corners gives none. */
 int ldso_b200_make_new_traces(ldso_b200_ctx *ctx, int slot, int nFeatures, const float *B, ldso_b200_features *out);
+/* FullSystem::makeNewTraces with setting_pointSelection == 0 (FullSystem.cc:1284-1303): ldso_b200_select_pixels on `slot`, then, for
+ * the selected pixels in raster order inside [3, w-4) x [3, h-4), the ImmaturePoint constructor with my_type = the map value on the
+ * device, as immature_seed runs it. Pixels whose energyTH is not finite are dropped; the rest form the slot's segment, in the order
+ * LDSO builds the keyframe's features. out->n_selected is makeMaps' value (it counts pixels of row h-4, which give no feature);
+ * out->n and u / v / my_type are the features. The store grows as immature_seed grows it. Errors as select_pixels, with the
+ * capacity checked against n_selected; a refused call leaves the segment as it was. */
+typedef struct ldso_b200_pixel_traces {
+    int capacity;                   /* rows of u / v / my_type: at least n_selected (w*h always suffices) */
+    int n_selected;                 /* out: makeMaps' return value */
+    int n;                          /* out: features, i.e. entries of the slot's segment */
+    float *u, *v, *my_type;
+} ldso_b200_pixel_traces;
+int ldso_b200_make_new_traces_pixels(ldso_b200_ctx *ctx, int slot, const ldso_b200_pixsel_params *params, const float *B,
+                                     int *current_potential, ldso_b200_pixel_traces *out);
 /* The ImmaturePoint constructor for n coordinates the caller already has (my_type may be NULL: type 1). Replaces the slot's segment.
  * LDSO_B200_ERR_ARG for a slot out of range or never filled, or a coordinate whose pattern leaves the image (2 <= u < w-3,
  * 2 <= v < h-3); a refused call leaves the segment as it was. Seeding any count succeeds whatever is live: the store grows. */

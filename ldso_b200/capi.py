@@ -89,6 +89,37 @@ class ImmatureSegmentC(C.Structure):
                 ("lastTraceUV2", c_fp), ("lastTracePixelInterval", c_fp), ("live", c_bp)]
 
 
+class PixselParamsC(C.Structure):
+    _fields_ = [("density", C.c_float), ("recursions_left", C.c_int), ("th_factor", C.c_float), ("minGradHistCut", C.c_float),
+                ("minGradHistAdd", C.c_float), ("gradDownweightPerLevel", C.c_float), ("selectDirectionDistribution", C.c_int)]
+
+
+class PixelsC(C.Structure):
+    _fields_ = [("capacity", C.c_int), ("n", C.c_int), ("n2", C.c_int), ("n3", C.c_int), ("n4", C.c_int), ("x", c_ip), ("y", c_ip),
+                ("type", c_bp), ("map", c_bp)]
+
+
+class PixelTracesC(C.Structure):
+    _fields_ = [("capacity", C.c_int), ("n_selected", C.c_int), ("n", C.c_int), ("u", c_fp), ("v", c_fp), ("my_type", c_fp)]
+
+
+def pixsel_params(density=1500.0, recursions_left=1, th_factor=1.0, minGradHistCut=0.5, minGradHistAdd=7.0, gradDownweightPerLevel=0.75,
+                  selectDirectionDistribution=1) -> PixselParamsC:
+    """ldso_b200_pixsel_params; the defaults are LDSO's settings and makeMaps' default arguments (FullSystem's call). The monocular
+    initializer's level-0 call is density=0.03*w*h, th_factor=2 with a current potential of 3."""
+    return PixselParamsC(float(density), int(recursions_left), float(th_factor), float(minGradHistCut), float(minGradHistAdd),
+                         float(gradDownweightPerLevel), int(selectDirectionDistribution))
+
+
+def pixsel_pattern(n) -> np.ndarray:
+    """ldso_b200_pixsel_pattern: the first n bytes of PixelSelector's randomPattern as the library generates them."""
+    out = np.zeros(max(int(n), 1), np.uint8)
+    r = load().ldso_b200_pixsel_pattern(int(n), out.ctypes.data_as(c_bp))
+    if r != 0:
+        raise Error(f"ldso_b200_pixsel_pattern({n}) failed: {r}")
+    return out[:int(n)]
+
+
 FEATURE_VALID, FEATURE_OUTLIER = 1, 2          # LDSO_B200_FEATURE_*
 
 
@@ -97,7 +128,8 @@ SYMBOLS = [
     "ldso_b200_default_settings", "ldso_b200_create", "ldso_b200_destroy", "ldso_b200_last_error", "ldso_b200_set_stream",
     "ldso_b200_synchronize", "ldso_b200_launch_count", "ldso_b200_kernel_times", "ldso_b200_upload_frame", "ldso_b200_make_images",
     "ldso_b200_download_frame_level", "ldso_b200_set_undistort", "ldso_b200_undistort_frame",
-    "ldso_b200_set_orb_pattern", "ldso_b200_feature_capacity", "ldso_b200_detect_corners", "ldso_b200_set_window", "ldso_b200_set_frames", "ldso_b200_set_marg_prior",
+    "ldso_b200_set_orb_pattern", "ldso_b200_feature_capacity", "ldso_b200_detect_corners", "ldso_b200_select_pixels", "ldso_b200_pixsel_pattern",
+    "ldso_b200_set_window", "ldso_b200_set_frames", "ldso_b200_set_marg_prior",
     "ldso_b200_get_marg_prior", "ldso_b200_linearize_all", "ldso_b200_apply_res", "ldso_b200_backup_state",
     "ldso_b200_solve_system", "ldso_b200_get_system", "ldso_b200_do_step", "ldso_b200_marginalize_points", "ldso_b200_marginalize_frame", "ldso_b200_calc_energies", "ldso_b200_accumulate", "ldso_b200_select_activation", "ldso_b200_init_calc_res", "ldso_b200_optimize_begin",
     "ldso_b200_gn_iterations", "ldso_b200_gn_iterations_until", "ldso_b200_get_iterations_run", "ldso_b200_get_until_form",
@@ -110,7 +142,7 @@ SYMBOLS = [
     "ldso_b200_tracker_set_ref_level", "ldso_b200_tracker_make_coarse_depth", "ldso_b200_tracker_get_ref_level",
     "ldso_b200_tracker_set_frames", "ldso_b200_tracker_eval", "ldso_b200_tracker_track", "ldso_b200_tracker_track_batch", "ldso_b200_posegraph_optimize",
     "ldso_b200_make_new_traces", "ldso_b200_immature_seed", "ldso_b200_trace_new_coarse", "ldso_b200_activate_immature",
-    "ldso_b200_immature_release", "ldso_b200_immature_read",
+    "ldso_b200_immature_release", "ldso_b200_immature_read", "ldso_b200_make_new_traces_pixels",
 ]
 
 _lib = None
@@ -138,6 +170,9 @@ def load():
         L.ldso_b200_feature_capacity.argtypes = [C.c_int, C.c_int, C.c_int]
         L.ldso_b200_detect_corners.argtypes = [C.c_void_p, C.c_int, C.c_int, c_fp, C.POINTER(FeaturesC)]
         L.ldso_b200_make_new_traces.argtypes = [C.c_void_p, C.c_int, C.c_int, c_fp, C.POINTER(FeaturesC)]
+        L.ldso_b200_select_pixels.argtypes = [C.c_void_p, C.c_int, C.POINTER(PixselParamsC), c_fp, c_ip, C.POINTER(PixelsC)]
+        L.ldso_b200_pixsel_pattern.argtypes = [C.c_int, c_bp]
+        L.ldso_b200_make_new_traces_pixels.argtypes = [C.c_void_p, C.c_int, C.POINTER(PixselParamsC), c_fp, c_ip, C.POINTER(PixelTracesC)]
         L.ldso_b200_immature_seed.argtypes = [C.c_void_p, C.c_int, C.c_int, c_fp, c_fp, c_fp]
         L.ldso_b200_trace_new_coarse.argtypes = [C.c_void_p, C.c_int, C.c_int, c_ip, c_fp, c_fp, c_fp, c_ip]
         L.ldso_b200_activate_immature.argtypes = [C.c_void_p, C.c_float, C.c_float, c_bp, C.c_int, C.POINTER(ActivationOutC)]
@@ -330,6 +365,46 @@ class Context:
         self._chk(fn(self.ctx, int(slot), int(n_features), _f(Bc), C.byref(f)))
         out = {k: a[:f.n] for k, a in o.items()}
         out["n_corners"] = int(f.n_corners)
+        return out
+
+    # ---- keyframe candidate pixels (PixelSelector::makeMaps on the device)
+    @staticmethod
+    def _pixsel_args(params, B, current_potential):
+        p = pixsel_params() if params is None else params
+        Bc = None
+        if B is not None:
+            Bc = np.ascontiguousarray(B, np.float32).reshape(-1)
+            if Bc.size != 256:
+                raise ValueError(f"B has {Bc.size} entries, expected 256")
+        return p, Bc, C.c_int(int(current_potential))
+
+    def select_pixels(self, slot, params=None, B=None, current_potential=3, capacity=None, want_map=False) -> dict:
+        """ldso_b200_select_pixels: makeMaps on the pyramid in `slot` (params: pixsel_params(), default FullSystem's call). Returns the
+        selected pixels in raster order (x, y, type), n, n2 / n3 / n4 of the final pass, current_potential as makeMaps leaves it, and
+        with want_map the w x h uint8 map. capacity defaults to w*h, which always suffices."""
+        p, Bc, pot = self._pixsel_args(params, B, current_potential)
+        cap = int(self.w * self.h if capacity is None else capacity)
+        o = dict(x=np.zeros(max(cap, 1), np.int32), y=np.zeros(max(cap, 1), np.int32), type=np.zeros(max(cap, 1), np.uint8))
+        mp = np.zeros((self.h, self.w), np.uint8) if want_map else None
+        s = PixelsC(cap, 0, 0, 0, 0, _i(o["x"]), _i(o["y"]), _b(o["type"]), _b(mp))
+        self._chk(self.L.ldso_b200_select_pixels(self.ctx, int(slot), C.byref(p), _f(Bc), C.byref(pot), C.byref(s)))
+        out = {k: a[:s.n] for k, a in o.items()}
+        out.update(n=int(s.n), n2=int(s.n2), n3=int(s.n3), n4=int(s.n4), current_potential=int(pot.value))
+        if want_map:
+            out["map"] = mp
+        return out
+
+    def make_new_traces_pixels(self, slot, params=None, B=None, current_potential=3, capacity=None) -> dict:
+        """ldso_b200_make_new_traces_pixels: makeNewTraces with setting_pointSelection == 0 into the slot's segment. Returns the
+        features (u, v, my_type) and their count n, n_selected (makeMaps' value) and current_potential. capacity defaults to w*h."""
+        p, Bc, pot = self._pixsel_args(params, B, current_potential)
+        cap = int(self.w * self.h if capacity is None else capacity)
+        o = dict(u=np.zeros(max(cap, 1), np.float32), v=np.zeros(max(cap, 1), np.float32), my_type=np.zeros(max(cap, 1), np.float32))
+        s = PixelTracesC(cap, 0, 0, _f(o["u"]), _f(o["v"]), _f(o["my_type"]))
+        self._chk(self.L.ldso_b200_make_new_traces_pixels(self.ctx, int(slot), C.byref(p), _f(Bc), C.byref(pot), C.byref(s)))
+        self._imm_rows[int(slot)] = int(s.n)
+        out = {k: a[:s.n] for k, a in o.items()}
+        out.update(n=int(s.n), n_selected=int(s.n_selected), current_potential=int(pot.value))
         return out
 
     # ---- the immature-point store (one segment per image slot, resident between calls)

@@ -24,6 +24,7 @@
 #include "finish.cuh"
 #include "undistort.cuh"
 #include "corners.cuh"
+#include "pixsel.cuh"
 
 static_assert(K1_THREADS / 32 == MAXF, "phase B maps one warp to one target frame");
 
@@ -59,6 +60,9 @@ struct ldso_b200_ctx {
     bool have_orb_pattern = false;
     float *corner_B = nullptr;
     char *corner_mem = nullptr, *corner_pin = nullptr;
+    // keyframe candidate pixels (select_pixels / make_new_traces_pixels): device block and pinned read-back block, allocated on
+    // first use (pixsel_layout); randomPattern is uploaded once, with the block
+    char *pix_mem = nullptr, *pix_pin = nullptr;
 
     // window
     DevWindow d;
@@ -365,6 +369,8 @@ extern "C" void ldso_b200_destroy(ldso_b200_ctx *c) {
     free_undistort(c);
     if (c->corner_mem) cudaFree(c->corner_mem);
     if (c->corner_pin) cudaFreeHost(c->corner_pin);
+    if (c->pix_mem) cudaFree(c->pix_mem);
+    if (c->pix_pin) cudaFreeHost(c->pix_pin);
     if (c->ws_dev) cudaFree(c->ws_dev);
     if (c->ws_host) cudaFreeHost(c->ws_host);
     if (c->sol_host) cudaFreeHost(c->sol_host);
@@ -688,6 +694,198 @@ extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeature
     CornerArgs a;
     RET_IF(corners_launch(c, slot, nFeatures, B, out, a));
     return corners_read(c, a, out);
+}
+
+// ---------------------------------------------------------------------------------------------- keyframe candidate pixels (pixsel.cuh)
+// select_pixels' device block, sized for what any potential needs (potential 1: one pot cell per pixel): the header, B,
+// randomPattern, the map, the cells' direction indices and masks, ths / thsSmoothed, the row counts and offsets, the raster list and
+// the output lists (x, y as int32 and type as uint8 for select_pixels, or u, v, my_type as floats for make_new_traces_pixels, in the
+// same bytes). The pinned block takes the header (64 bytes), then the lists and the map.
+struct PixselLayout { size_t hdr, B, rp, map, dir, mask, ths, thsS, rowcnt, rowoff, list, out, total, pin; };
+static PixselLayout pixsel_layout(int w, int h) {
+    const size_t px = (size_t) w * h, cells = (size_t) (w / 32) * (h / 32);
+    PixselLayout L;
+    size_t o = 0;
+    L.hdr = o; o += align16(4 * PIXSEL_HDR_INTS);
+    L.B = o; o += align16(4 * 256);
+    L.rp = o; o += align16(px);
+    L.map = o; o += align16(px);
+    L.dir = o; o += align16(px);
+    L.mask = o; o += align16(2 * px);
+    L.ths = o; o += align16(4 * cells);
+    L.thsS = o; o += align16(4 * cells);
+    L.rowcnt = o; o += align16(4 * (size_t) h);
+    L.rowoff = o; o += align16(4 * (size_t) h);
+    L.list = o; o += align16(4 * px);
+    L.out = o; o += 12 * px;
+    L.total = o;
+    L.pin = 64 + 12 * px;
+    return L;
+}
+
+// PixelSelector's randomPattern (PixelSelector2.cc:11-13): rand() & 0xFF after srand(3141592). glibc's rand() is random() on a
+// TYPE_3 state of 128 bytes; initstate_r seeds a private state of that type exactly as srand seeds the global one, so the caller's
+// rand() sequence is left alone.
+static void pixsel_pattern(uint8_t *out, size_t n) {
+    struct random_data rd;
+    memset(&rd, 0, sizeof(rd));
+    char state[128];
+    initstate_r(3141592, state, sizeof(state), &rd);
+    for (size_t i = 0; i < n; i++) {
+        int32_t r;
+        random_r(&rd, &r);
+        out[i] = (uint8_t) (r & 0xFF);
+    }
+}
+
+extern "C" int ldso_b200_pixsel_pattern(int n, uint8_t *out) {
+    if (n < 0 || (n > 0 && !out)) return LDSO_B200_ERR_ARG;
+    pixsel_pattern(out, (size_t) n);
+    return LDSO_B200_OK;
+}
+
+static int pixsel_ensure(ldso_b200_ctx *c) {
+    if (c->pix_mem) return LDSO_B200_OK;
+    const PixselLayout L = pixsel_layout(c->w, c->h);
+    char *m = nullptr, *pin = nullptr;
+    cudaError_t e = cudaMalloc(&m, L.total);
+    if (e == cudaSuccess) e = cudaMallocHost(&pin, L.pin);
+    if (e == cudaSuccess) {
+        pixsel_pattern((uint8_t *) pin, (size_t) c->w * c->h);
+        e = cudaMemcpy(m + L.rp, pin, (size_t) c->w * c->h, cudaMemcpyHostToDevice);
+    }
+    if (e != cudaSuccess) {
+        if (m) cudaFree(m);
+        if (pin) cudaFreeHost(pin);
+        return c->fail_cuda(e, "pixel selection scratch", __FILE__, __LINE__);
+    }
+    c->pix_mem = m; c->pix_pin = pin;
+    return LDSO_B200_OK;
+}
+
+// float -> int as the reference's x86 build converts (cvttss2si): truncation, INT_MIN for NaN and out-of-range values
+static int pixsel_f2i(float f) { return (f >= -2147483648.f && f < 2147483648.f) ? (int) f : INT_MIN; }
+
+struct PixselResult { int n2, n3, n4, nsel, nkept, nfeat, pot; };
+
+// makeMaps (PixelSelector2.cc:111-168) up to the output lists: the histogram once, one select() pass per recursion with a 16-byte
+// read-back of its counts, the recursion and currentPotential on the host with the reference's float arithmetic, then the
+// subsampling and the lists: every kept pixel as x / y / type, or (traces) the kept pixels in makeNewTraces' range as u / v / my_type.
+// Ends with the header on the host.
+static int pixsel_run(ldso_b200_ctx *c, const char *what, int slot, const ldso_b200_pixsel_params *p, const float *B, const int *current_potential,
+                      bool traces, PixselArgs &a, PixselResult &R) {
+    char msg[160];
+#define PIXSEL_FAIL(text) do { snprintf(msg, sizeof(msg), "%s: %s", what, text); return c->fail(LDSO_B200_ERR_ARG, msg); } while (0)
+    if (c->levels < 3) PIXSEL_FAIL("needs a context with at least 3 pyramid levels");
+    if (slot < 0 || slot >= NSLOTS || !c->img[slot][0]) PIXSEL_FAIL("image slot out of range or never filled");
+    if (!p || !current_potential) PIXSEL_FAIL("params or current_potential is NULL");
+    if (!(p->density > 0)) PIXSEL_FAIL("density must be positive");
+    if (*current_potential < 1) PIXSEL_FAIL("current_potential must be at least 1");
+#undef PIXSEL_FAIL
+    cudaSetDevice(c->device);
+    RET_IF(pixsel_ensure(c));
+    const int w = c->w, h = c->h;
+    const size_t px = (size_t) w * h;
+    const PixselLayout L = pixsel_layout(w, h);
+    char *m = c->pix_mem;
+    a.img0 = c->img[slot][0]; a.img1 = c->img[slot][1]; a.img2 = c->img[slot][2];
+    a.B = nullptr;
+    if (B) {
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(m + L.B, B, sizeof(float) * 256, cudaMemcpyHostToDevice, c->stream));
+        a.B = (const float *) (m + L.B);
+    }
+    a.w = w; a.h = h; a.w1 = c->lw[1]; a.w2 = c->lw[2];
+    a.w32 = w / 32; a.h32 = h / 32;
+    a.minGradHistCut = p->minGradHistCut; a.minGradHistAdd = p->minGradHistAdd;
+    a.ths = (float *) (m + L.ths); a.thsS = (float *) (m + L.thsS);
+    a.rp = (const uint8_t *) (m + L.rp);
+    a.thFactor = p->th_factor; a.dw1 = p->gradDownweightPerLevel; a.dw2 = a.dw1 * a.dw1;
+    a.dirDist = p->selectDirectionDistribution != 0;
+    a.mask = (uint16_t *) (m + L.mask); a.dir = (uint8_t *) (m + L.dir); a.map = (uint8_t *) (m + L.map);
+    a.hdr = (int *) (m + L.hdr);
+    a.rowcnt = (int *) (m + L.rowcnt); a.rowoff = (int *) (m + L.rowoff); a.list = (int *) (m + L.list);
+    a.sx = a.sy = nullptr; a.stype = nullptr; a.fu = a.fv = a.ftype = nullptr;
+    if (traces) { a.fu = (float *) (m + L.out); a.fv = a.fu + px; a.ftype = a.fv + px; }
+    else { a.sx = (int32_t *) (m + L.out); a.sy = a.sx + px; a.stype = (uint8_t *) (a.sy + px); }
+    const int ncell32 = a.w32 * a.h32;
+    if (ncell32 > 0) {                  // makeHists: once per call, whatever the potential
+        k_pixsel_hist<<<ncell32, 1024, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+        k_pixsel_smooth<<<(ncell32 + 255) / 256, 256, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+    }
+    int pot = *current_potential, rec = p->recursions_left, ideal = pot;
+    float quotia = 0.f;
+    const int *hh = (const int *) c->pix_pin;
+    for (;;) {
+        // a potential of max(w, h) or more gives one cell, one 2pot and one 4pot block covering the image: the same pass
+        const int pg = std::min(pot, std::max(w, h));
+        a.pot = pg; a.cw = (w + pg - 1) / pg; a.ch = (h + pg - 1) / pg; a.bw4 = (w + 4 * pg - 1) / (4 * pg); a.bh4 = (h + 4 * pg - 1) / (4 * pg);
+        CUDA_CHECK_RET(c, cudaMemsetAsync(a.map, 0, px, c->stream));
+        CUDA_CHECK_RET(c, cudaMemsetAsync(a.hdr, 0, 4 * PIXSEL_HDR_INTS, c->stream));
+        k_pixsel_mask<<<(a.cw * a.ch + 255) / 256, 256, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+        k_pixsel_walk<<<1, 32, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+        k_pixsel_pick<<<(a.bw4 * a.bh4 + 127) / 128, 128, 0, c->stream>>>(a);
+        LAUNCH_CHECK(c);
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(c->pix_pin, a.hdr, 16, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+        R.n2 = hh[PIXSEL_N2]; R.n3 = hh[PIXSEL_N3]; R.n4 = hh[PIXSEL_N4];
+        const float numHave = (float) (R.n2 + R.n3 + R.n4), numWant = p->density;
+        quotia = numWant / numHave;
+        const float K = numHave * (pot + 1) * (pot + 1);
+        ideal = pixsel_f2i(sqrtf(K / numWant) - 1);
+        if (ideal < 1) ideal = 1;
+        if (rec > 0 && quotia > 1.25 && pot > 1) {
+            if (ideal >= pot) ideal = pot - 1;
+            pot = ideal; rec--;
+        } else if (rec > 0 && quotia < 0.25) {
+            if (ideal <= pot) ideal = pot + 1;
+            pot = ideal; rec--;
+        } else {
+            break;
+        }
+    }
+    a.charTH = quotia < 0.95 ? (int) (unsigned char) (255 * quotia) : 255;
+    const int rows = (h * 32 + 255) / 256;
+    k_pixsel_rows<<<rows, 256, 0, c->stream>>>(a);
+    LAUNCH_CHECK(c);
+    k_pixsel_row_scan<<<1, 1024, 0, c->stream>>>(a);
+    LAUNCH_CHECK(c);
+    k_pixsel_emit<<<rows, 256, 0, c->stream>>>(a);
+    LAUNCH_CHECK(c);
+    k_pixsel_finish<<<1, 1024, 0, c->stream>>>(a);
+    LAUNCH_CHECK(c);
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->pix_pin, a.hdr, 64, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    R.nsel = hh[PIXSEL_NSEL]; R.nkept = hh[PIXSEL_NKEPT]; R.nfeat = hh[PIXSEL_NFEAT]; R.pot = ideal;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_select_pixels(ldso_b200_ctx *c, int slot, const ldso_b200_pixsel_params *params, const float *B, int *current_potential,
+                                       ldso_b200_pixels *out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    if (!out || !out->x || !out->y || !out->type) return c->fail(LDSO_B200_ERR_ARG, "select_pixels: missing output array");
+    PixselArgs a;
+    PixselResult R;
+    RET_IF(pixsel_run(c, "select_pixels", slot, params, B, current_potential, false, a, R));
+    const size_t px = (size_t) c->w * c->h;
+    const int n = R.nkept;
+    if (out->capacity < n) return c->fail(LDSO_B200_ERR_ARG, "select_pixels: capacity below the number of selected pixels");
+    char *q = c->pix_pin + 64;
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(q, a.sx, 4 * (size_t) n, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 4 * (size_t) n, a.sy, 4 * (size_t) n, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 8 * (size_t) n, a.stype, (size_t) n, cudaMemcpyDeviceToHost, c->stream));
+    if (out->map) CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 9 * (size_t) n, a.map, px, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+    memcpy(out->x, q, 4 * (size_t) n);
+    memcpy(out->y, q + 4 * (size_t) n, 4 * (size_t) n);
+    memcpy(out->type, q + 8 * (size_t) n, (size_t) n);
+    if (out->map) memcpy(out->map, q + 9 * (size_t) n, px);
+    out->n = n; out->n2 = R.n2; out->n3 = R.n3; out->n4 = R.n4;
+    *current_potential = R.pot;
+    return LDSO_B200_OK;
 }
 
 extern "C" int ldso_b200_download_frame_level(ldso_b200_ctx *c, int slot, int lvl, float *out) {
@@ -1697,6 +1895,44 @@ extern "C" int ldso_b200_immature_seed(ldso_b200_ctx *c, int slot, int n, const 
     LAUNCH_CHECK(c);
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     c->imm_n[slot] = c->imm_live[slot] = n;
+    return LDSO_B200_OK;
+}
+
+extern "C" int ldso_b200_make_new_traces_pixels(ldso_b200_ctx *c, int slot, const ldso_b200_pixsel_params *params, const float *B,
+                                                int *current_potential, ldso_b200_pixel_traces *out) {
+    if (!c) return LDSO_B200_ERR_ARG;
+    IMM_SINGLE(c, "make_new_traces_pixels");
+    if (!out || !out->u || !out->v || !out->my_type) return c->fail(LDSO_B200_ERR_ARG, "make_new_traces_pixels: missing output array");
+    PixselArgs a;
+    PixselResult R;
+    RET_IF(pixsel_run(c, "make_new_traces_pixels", slot, params, B, current_potential, true, a, R));
+    if (out->capacity < R.nkept) return c->fail(LDSO_B200_ERR_ARG, "make_new_traces_pixels: capacity below the number of selected pixels");
+    const int nf = R.nfeat;
+    RET_IF(imm_reserve(c, nf));
+    c->imm_n[slot] = c->imm_live[slot] = 0;
+    int n = 0;
+    if (nf > 0) {
+        // the constructor for every pixel in range, then the entries whose energyTH is not finite leave the segment
+        launch_store_seed(nullptr, nf, a.fu, a.fv, a.ftype, c->img[slot][0], c->w, trace_settings(c), c->imm_store, c->imm_cap, slot, c->stream);
+        LAUNCH_CHECK(c);
+        launch_store_compact(c->imm_store, c->imm_cap, slot, nf, a.hdr + PIXSEL_NSEED, c->stream);
+        LAUNCH_CHECK(c);
+        const ImmSeg g = imm_seg(c->imm_store, c->imm_cap, slot);
+        char *q = c->pix_pin;
+        const size_t N = (size_t) nf;
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(q, a.hdr, 64, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 64, g.u, 4 * N, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 64 + 4 * N, g.v, 4 * N, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 64 + 8 * N, g.my_type, 4 * N, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
+        n = ((const int *) q)[PIXSEL_NSEED];
+        memcpy(out->u, q + 64, 4 * (size_t) n);
+        memcpy(out->v, q + 64 + 4 * N, 4 * (size_t) n);
+        memcpy(out->my_type, q + 64 + 8 * N, 4 * (size_t) n);
+    }
+    c->imm_n[slot] = c->imm_live[slot] = n;
+    out->n_selected = R.nkept; out->n = n;
+    *current_potential = R.pot;
     return LDSO_B200_OK;
 }
 

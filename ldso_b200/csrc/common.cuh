@@ -179,3 +179,23 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
         cudaError_t e__ = (call);                                                         \
         if (e__ != cudaSuccess) return (ctx)->fail_cuda(e__, #call, __FILE__, __LINE__);  \
     } while (0)
+
+// exclusive prefix sum over a 1024-thread block; *total gets the block's sum (s holds 33 ints)
+__device__ __forceinline__ int imm_block_scan(int x, int *s, int *total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int inc = x;
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+    if (lane == 31) s[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+        int t = s[lane], ti = t;
+        for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, ti, o); if (lane >= o) ti += y; }
+        s[lane] = ti - t;
+        if (lane == 31) s[32] = ti;
+    }
+    __syncthreads();
+    const int r = s[warp] + inc - x;
+    *total = s[32];
+    __syncthreads();
+    return r;
+}

@@ -11,6 +11,7 @@
 //                      and the ORB descriptor of every surviving corner (atan2 / cos / sin in double, rounded to float)
 #pragma once
 #include "common.cuh"
+#include "img_kernels.cuh"
 
 #define CORNER_HALF_PATCH 15
 #define CORNER_THREADS 256
@@ -38,18 +39,7 @@ struct CornerArgs {
     uint8_t *is_corner, *desc;
 };
 
-__device__ __forceinline__ float corner_grad(const CornerArgs &a, int idx) {
-    const float4 t = a.img[idx];
-    float g = __fadd_rn(__fmul_rn(t.y, t.y), __fmul_rn(t.z, t.z));
-    if (a.B) {
-        int c = (int) __fadd_rn(t.x, 0.5f);            // CalibHessian::getBGradOnly
-        if (c < 5) c = 5;
-        if (c > 250) c = 250;
-        const float gw = __fsub_rn(__ldg(a.B + c + 1), __ldg(a.B + c));
-        g = __fmul_rn(g, __fmul_rn(gw, gw));
-    }
-    return g;
-}
+__device__ __forceinline__ float corner_grad(const CornerArgs &a, int idx) { return pyr_abs_sq_grad(a.img, a.B, idx); }
 
 __device__ float corner_shi_tomasi(const CornerArgs &a, int u, int v) {
     const int x_min = u - 4, x_max = u + 4, y_min = v - 4, y_max = v + 4;

@@ -41,3 +41,20 @@ __global__ void k_pyr_level(const float *__restrict__ color, const float4 *__res
     }
     dst[idx] = make_float4(v, dx, dy, 0.f);
 }
+
+// absSquaredGrad[l][idx] as makeImages forms it (FrameHessian.cc:91-97) from a level-l texel: dx^2 + dy^2, times the square of
+// CalibHessian::getBGradOnly(I) when B is given (nullptr = identity, setting_gammaWeightsPixelSelect = 1). Each product and sum is
+// rounded on its own. On a pyramid built here (k_pyr_level) rows 0 and h_l-1, which makeImages never writes, give 0: their texels
+// hold dx = dy = 0.
+__device__ __forceinline__ float pyr_abs_sq_grad(const float4 *img, const float *B, int idx) {
+    const float4 t = img[idx];
+    float g = __fadd_rn(__fmul_rn(t.y, t.y), __fmul_rn(t.z, t.z));
+    if (B) {
+        int c = (int) __fadd_rn(t.x, 0.5f);            // CalibHessian::getBGradOnly
+        if (c < 5) c = 5;
+        if (c > 250) c = 250;
+        const float gw = __fsub_rn(__ldg(B + c + 1), __ldg(B + c));
+        g = __fmul_rn(g, __fmul_rn(gw, gw));
+    }
+    return g;
+}

@@ -7,26 +7,6 @@
 #include "trace_kernels.cuh"
 #include "immature_store.h"
 
-// exclusive prefix sum over a 1024-thread block; *total gets the block's sum (s holds 33 ints)
-__device__ __forceinline__ int imm_block_scan(int x, int *s, int *total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int inc = x;
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-    if (lane == 31) s[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-        int t = s[lane], ti = t;
-        for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, ti, o); if (lane >= o) ti += y; }
-        s[lane] = ti - t;
-        if (lane == 31) s[32] = ti;
-    }
-    __syncthreads();
-    const int r = s[warp] + inc - x;
-    *total = s[32];
-    __syncthreads();
-    return r;
-}
-
 // The ImmaturePoint constructor for entries 0..n-1 of a segment (n from n_dev when given): u, v and my_type are copied in from src_*
 // (my_type 1 when src_type is null; the sources may be the segment's own arrays), then the fresh trace state: idepth_min 0,
 // idepth_max NaN, quality 10000, UNINITIALIZED (ImmaturePoint.h:103-121).
@@ -41,6 +21,41 @@ __global__ void k_store_seed(const int *n_dev, int n, const float *src_u, const 
     immature_init_one(i, img, w, g.u, g.v, S, g.color8, g.weights8, g.gradH4, g.energyTH);
     g.idmin[i] = 0.f; g.idmax[i] = NAN; g.quality[i] = 10000.f; g.status[i] = IPS_UNINITIALIZED;
     g.uv2[2 * i] = 0.f; g.uv2[2 * i + 1] = 0.f; g.interval[i] = 0.f; g.live[i] = 1;
+}
+
+// makeNewTraces' energyTH check (FullSystem.cc:1298-1302): entries 0..n-1 of a freshly seeded segment whose energyTH is not finite
+// are dropped, the others move down in order; *n_out gets the count kept. One CTA, in rounds of 1024 entries: a round reads its
+// entries before any of them is written, and an entry only ever moves to a lower index, so no entry is overwritten before it moved.
+__global__ void __launch_bounds__(1024) k_store_compact(float *store, int cap, int slot, int n, int *n_out) {
+    __shared__ int s[33];
+    const ImmSeg g = imm_seg(store, cap, slot);
+    float *const f1[] = {g.u, g.v, g.my_type, g.energyTH, g.idmin, g.idmax, g.quality, (float *) g.status, g.interval, (float *) g.live};
+    int o = 0;
+    for (int r0 = 0; r0 < n; r0 += 1024) {
+        const int i = r0 + threadIdx.x;
+        const bool keep = i < n && isfinite(g.energyTH[i]);
+        int tot;
+        const int d = o + imm_block_scan(keep, s, &tot);
+        if (o != r0 || tot != min(1024, n - r0)) {       // something moves in this round
+            float r[IMM_SEG_WORDS];
+            if (keep) {
+                for (int k = 0; k < 10; k++) r[k] = f1[k][i];
+                for (int k = 0; k < 8; k++) { r[10 + k] = g.color8[8 * i + k]; r[18 + k] = g.weights8[8 * i + k]; }
+                for (int k = 0; k < 4; k++) r[26 + k] = g.gradH4[4 * i + k];
+                r[30] = g.uv2[2 * i]; r[31] = g.uv2[2 * i + 1];
+            }
+            __syncthreads();
+            if (keep) {
+                for (int k = 0; k < 10; k++) f1[k][d] = r[k];
+                for (int k = 0; k < 8; k++) { g.color8[8 * d + k] = r[10 + k]; g.weights8[8 * d + k] = r[18 + k]; }
+                for (int k = 0; k < 4; k++) g.gradH4[4 * d + k] = r[26 + k];
+                g.uv2[2 * d] = r[30]; g.uv2[2 * d + 1] = r[31];
+            }
+            __syncthreads();
+        }
+        o += tot;
+    }
+    if (threadIdx.x == 0) *n_out = o;
 }
 
 // One traceNewCoarse pass over the listed segments: warp w takes entry w - begin[j] of segment j, skips it when it is not live, and

@@ -59,6 +59,7 @@ struct StoreActArgs {
 
 void launch_store_seed(const int *n_dev, int n, const float *src_u, const float *src_v, const float *src_type, const float4 *img, int w,
                        const TraceSettingsDev &S, float *store, int cap, int slot, cudaStream_t stream);
+void launch_store_compact(float *store, int cap, int slot, int n, int *n_out, cudaStream_t stream);
 void launch_store_trace(const StoreTraceArgs &P, cudaStream_t stream);
 void launch_store_gather(const StoreActArgs &P, cudaStream_t stream);
 void launch_store_pick(const StoreActArgs &P, cudaStream_t stream);

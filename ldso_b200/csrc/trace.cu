@@ -31,6 +31,9 @@ void launch_store_seed(const int *n_dev, int n, const float *src_u, const float 
                        const TraceSettingsDev &S, float *store, int cap, int slot, cudaStream_t stream) {
     k_store_seed<<<(n + 127) / 128, 128, 0, stream>>>(n_dev, n, src_u, src_v, src_type, img, w, S, store, cap, slot);
 }
+void launch_store_compact(float *store, int cap, int slot, int n, int *n_out, cudaStream_t stream) {
+    k_store_compact<<<1, 1024, 0, stream>>>(store, cap, slot, n, n_out);
+}
 void launch_store_trace(const StoreTraceArgs &P, cudaStream_t stream) {
     k_store_trace<<<(P.begin[P.nseg] + KTR_WARPS - 1) / KTR_WARPS, 32 * KTR_WARPS, 0, stream>>>(P);
 }
