@@ -25,6 +25,7 @@
 #include "undistort.cuh"
 #include "corners.cuh"
 #include "pixsel.cuh"
+#include "scratch_layout.cuh"
 
 static_assert(K1_THREADS / 32 == MAXF, "phase B maps one warp to one target frame");
 
@@ -61,7 +62,7 @@ struct ldso_b200_ctx {
     float *corner_B = nullptr;
     char *corner_mem = nullptr, *corner_pin = nullptr;
     // keyframe candidate pixels (select_pixels / make_new_traces_pixels): device block and pinned read-back block, allocated on
-    // first use (pixsel_layout); randomPattern is uploaded once, with the block
+    // first use (pixsel_ensure); randomPattern is uploaded once, with the block
     char *pix_mem = nullptr, *pix_pin = nullptr;
 
     // window
@@ -72,7 +73,7 @@ struct ldso_b200_ctx {
     bool select_pending = false;     // the newest frame's energy threshold of the last fused iteration has not been computed yet (flush_select)
     bool has_lin = false;            // the window holds linearized (isLinearized) residuals: solve_system accumulates HA + HL in one pass
     std::vector<unsigned char> h_scratch_bytes;     // select_activation's map read-back
-    unsigned char *actsel_pin = nullptr; size_t actsel_pin_cap = 0;      // its pinned staging block
+    char *actsel_pin = nullptr; size_t actsel_pin_cap = 0;      // its pinned staging block
     std::vector<int> h_pt_host, h_res_begin, h_res_target;
     int nF = 0, n = 0;
     int slots[MAXF];
@@ -126,7 +127,7 @@ struct ldso_b200_ctx {
     bool use_pdl = true;             // programmatic dependent launch inside the GN iteration (env LDSO_B200_NO_PDL disables)
     bool pdl_now = false;            // set while launch_gn_body issues its four kernels
     size_t k1_smem = 0;
-    char *trace_buf = nullptr;       // device scratch of immature_init / trace_immature
+    char *trace_buf = nullptr;       // device scratch of the one-shot entry points (trace_carve)
     size_t trace_cap = 0;
     // immature-point store (immature_store.h): the segments (imm_cap entries each), activate_immature's scratch and the pinned
     // read-back block, allocated together on first use; per slot the entries seeded and how many of them are still live
@@ -230,28 +231,6 @@ extern "C" void ldso_b200_default_settings(ldso_b200_settings *s) {
     s->trace_GNIterations = 3;
 }
 
-// detect_corners' device block, sized for one feature per pixel (px = w*h): the output block first (n, scoreTH, then u | v | score |
-// angle | is_corner | descriptor, laid out per call with that call's capacity), then the ORB pattern, B and the per-cell scratch.
-// Every region starts on a 16-byte boundary whatever w*h is.
-struct CornerLayout { size_t out_bytes, pattern, B, keys, cell_count, cell_off, pick_px, cell_max, pick_score, initial, total; };
-static size_t align16(size_t n) { return (n + 15) & ~(size_t) 15; }
-static CornerLayout corner_layout(size_t px) {
-    CornerLayout L;
-    size_t o = 0;
-    L.out_bytes = align16(16 + px * CORNER_FEATURE_BYTES); o = L.out_bytes;
-    L.pattern = o; o = align16(o + 1024 * sizeof(int));
-    L.B = o; o = align16(o + 256 * sizeof(float));
-    L.keys = o; o = align16(o + px * sizeof(unsigned long long));
-    L.cell_count = o; o = align16(o + px * sizeof(int));
-    L.cell_off = o; o = align16(o + px * sizeof(int));
-    L.pick_px = o; o = align16(o + px * sizeof(int));
-    L.cell_max = o; o = align16(o + px * sizeof(float));
-    L.pick_score = o; o = align16(o + px * sizeof(float));
-    L.initial = o; o = align16(o + px);
-    L.total = o;
-    return L;
-}
-
 extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_levels, const ldso_b200_settings *settings) {
     if (w <= 0 || h <= 0 || pyr_levels < 1 || pyr_levels > MAXLVL) return nullptr;
     int ndev = 0;
@@ -306,11 +285,16 @@ extern "C" ldso_b200_ctx *ldso_b200_create(int device, int w, int h, int pyr_lev
     ok = cudaMallocHost(&c->sol_host, sizeof(double) * (nn + 3 * MAXN)) == cudaSuccess;      // [lastHS | lastbS | lastX | scalars]
     if (!ok) { fprintf(stderr, "ldso_b200: pinned allocation failed\n"); delete c; return nullptr; }
     {
-        const CornerLayout L = corner_layout((size_t) w * h);
-        ok = cudaMalloc(&c->corner_mem, L.total) == cudaSuccess && cudaMallocHost(&c->corner_pin, L.out_bytes) == cudaSuccess;
+        const size_t px = (size_t) w * h;
+        CornerArgs a;
+        Arena S;
+        corner_regions(S, px, 0, a);
+        ok = cudaMalloc(&c->corner_mem, S.off) == cudaSuccess && cudaMallocHost(&c->corner_pin, corner_out_bytes(px)) == cudaSuccess;
         if (!ok) { fprintf(stderr, "ldso_b200: corner scratch allocation failed\n"); delete c; return nullptr; }
-        c->orb_pattern = (int *) (c->corner_mem + L.pattern);
-        c->corner_B = (float *) (c->corner_mem + L.B);
+        Arena D(c->corner_mem);
+        const CornerFixed f = corner_regions(D, px, 0, a);
+        c->orb_pattern = f.pattern;
+        c->corner_B = f.B;
     }
     c->ktime = getenv("LDSO_B200_KTIME") != nullptr;
     c->use_graph = !c->ktime && getenv("LDSO_B200_NO_GRAPH") == nullptr;
@@ -424,6 +408,8 @@ extern "C" int ldso_b200_synchronize(ldso_b200_ctx *c) {
 
 #define RET_IF(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
 #define D2H(dst, src, bytes) do { if (dst) CUDA_CHECK_RET(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream)); } while (0)
+// dst may be a const member of a kernel's argument struct: the host fills what the kernel only reads
+#define H2D(dst, src, bytes) CUDA_CHECK_RET(c, cudaMemcpyAsync((void *) (dst), src, bytes, cudaMemcpyHostToDevice, c->stream))
 
 static int wait_results(ldso_b200_ctx *c);
 
@@ -614,11 +600,12 @@ static int corners_launch(ldso_b200_ctx *c, int slot, int nFeatures, const float
     const int cap = g.ncx * g.ncy * g.kcap;
     if (out->capacity < cap) return c->fail(LDSO_B200_ERR_ARG, "detect_corners: capacity below ldso_b200_feature_capacity(w, h, nFeatures)");
     cudaSetDevice(c->device);
-    const size_t px = (size_t) c->w * c->h;
+    Arena D(c->corner_mem);
+    corner_regions(D, (size_t) c->w * c->h, cap, a);
     a.img = c->img[slot][0];
     a.B = nullptr;
     if (B) {
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(c->corner_B, B, sizeof(float) * 256, cudaMemcpyHostToDevice, c->stream));
+        H2D(c->corner_B, B, sizeof(float) * 256);
         a.B = c->corner_B;
     }
     a.pattern = c->orb_pattern;
@@ -634,21 +621,6 @@ static int corners_launch(ldso_b200_ctx *c, int slot, int nFeatures, const float
             ++v0;
         }
     }
-    const CornerLayout L = corner_layout(px);
-    char *m = c->corner_mem;
-    a.keys = (unsigned long long *) (m + L.keys);
-    a.cell_count = (int *) (m + L.cell_count);
-    a.cell_off = (int *) (m + L.cell_off);
-    a.pick_px = (int *) (m + L.pick_px);
-    a.cell_max = (float *) (m + L.cell_max);
-    a.pick_score = (float *) (m + L.pick_score);
-    a.initial = (uint8_t *) (m + L.initial);
-    // the output block at the start, laid out with this call's capacity so that one copy brings it back
-    char *o = m;
-    a.hdr = (int *) o;
-    a.cap = cap;
-    a.u = (float *) (o + 16); a.v = a.u + cap; a.score = a.v + cap; a.angle = a.score + cap;
-    a.is_corner = (uint8_t *) (a.angle + cap); a.desc = a.is_corner + cap;
     const int ncell = g.ncx * g.ncy;
     if (ncell == 0) {
         CUDA_CHECK_RET(c, cudaMemsetAsync(a.hdr, 0, 16, c->stream));
@@ -667,23 +639,19 @@ static int corners_launch(ldso_b200_ctx *c, int slot, int nFeatures, const float
 }
 
 static int corners_read(ldso_b200_ctx *c, const CornerArgs &a, ldso_b200_features *out) {
-    const int cap = a.cap;
-    const size_t out_bytes = 16 + (size_t) cap * CORNER_FEATURE_BYTES;
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->corner_pin, a.hdr, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CornerArgs h;      // the output block's split, at the pinned copy
+    corner_split(c->corner_pin, a.cap, h);
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(h.hdr, a.hdr, corner_out_bytes(a.cap), cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
-    const char *q = c->corner_pin;
-    int n;
-    memcpy(&n, q, sizeof(int));
-    const float *hu = (const float *) (q + 16), *hv = hu + cap, *hs = hv + cap, *ha = hs + cap;
-    const uint8_t *hc = (const uint8_t *) (ha + cap), *hd = hc + cap;
-    memcpy(out->u, hu, sizeof(float) * n);
-    memcpy(out->v, hv, sizeof(float) * n);
-    memcpy(out->score, hs, sizeof(float) * n);
-    memcpy(out->angle, ha, sizeof(float) * n);
-    memcpy(out->is_corner, hc, n);
-    memcpy(out->descriptor, hd, (size_t) 32 * n);
+    const int n = h.hdr[0];
+    memcpy(out->u, h.u, sizeof(float) * n);
+    memcpy(out->v, h.v, sizeof(float) * n);
+    memcpy(out->score, h.score, sizeof(float) * n);
+    memcpy(out->angle, h.angle, sizeof(float) * n);
+    memcpy(out->is_corner, h.is_corner, n);
+    memcpy(out->descriptor, h.desc, (size_t) 32 * n);
     int nc = 0;
-    for (int i = 0; i < n; i++) nc += hc[i] != 0;
+    for (int i = 0; i < n; i++) nc += h.is_corner[i] != 0;
     out->n = n;
     out->n_corners = nc;
     return LDSO_B200_OK;
@@ -697,32 +665,6 @@ extern "C" int ldso_b200_detect_corners(ldso_b200_ctx *c, int slot, int nFeature
 }
 
 // ---------------------------------------------------------------------------------------------- keyframe candidate pixels (pixsel.cuh)
-// select_pixels' device block, sized for what any potential needs (potential 1: one pot cell per pixel): the header, B,
-// randomPattern, the map, the cells' direction indices and masks, ths / thsSmoothed, the row counts and offsets, the raster list and
-// the output lists (x, y as int32 and type as uint8 for select_pixels, or u, v, my_type as floats for make_new_traces_pixels, in the
-// same bytes). The pinned block takes the header (64 bytes), then the lists and the map.
-struct PixselLayout { size_t hdr, B, rp, map, dir, mask, ths, thsS, rowcnt, rowoff, list, out, total, pin; };
-static PixselLayout pixsel_layout(int w, int h) {
-    const size_t px = (size_t) w * h, cells = (size_t) (w / 32) * (h / 32);
-    PixselLayout L;
-    size_t o = 0;
-    L.hdr = o; o += align16(4 * PIXSEL_HDR_INTS);
-    L.B = o; o += align16(4 * 256);
-    L.rp = o; o += align16(px);
-    L.map = o; o += align16(px);
-    L.dir = o; o += align16(px);
-    L.mask = o; o += align16(2 * px);
-    L.ths = o; o += align16(4 * cells);
-    L.thsS = o; o += align16(4 * cells);
-    L.rowcnt = o; o += align16(4 * (size_t) h);
-    L.rowoff = o; o += align16(4 * (size_t) h);
-    L.list = o; o += align16(4 * px);
-    L.out = o; o += 12 * px;
-    L.total = o;
-    L.pin = 64 + 12 * px;
-    return L;
-}
-
 // PixelSelector's randomPattern (PixelSelector2.cc:11-13): rand() & 0xFF after srand(3141592). glibc's rand() is random() on a
 // TYPE_3 state of 128 bytes; initstate_r seeds a private state of that type exactly as srand seeds the global one, so the caller's
 // rand() sequence is left alone.
@@ -744,15 +686,23 @@ extern "C" int ldso_b200_pixsel_pattern(int n, uint8_t *out) {
     return LDSO_B200_OK;
 }
 
+// the device block (pixsel_regions) and the pinned block (pixsel_pin_regions), allocated on first use; randomPattern is uploaded once
 static int pixsel_ensure(ldso_b200_ctx *c) {
     if (c->pix_mem) return LDSO_B200_OK;
-    const PixselLayout L = pixsel_layout(c->w, c->h);
+    const size_t px = (size_t) c->w * c->h;
+    PixselArgs a;
+    Arena S, P, Q;
+    pixsel_regions(S, c->w, c->h, true, a);
+    pixsel_pin_regions(P, px, px, true, a);
+    pixsel_pin_regions(Q, px, px, false, a);
     char *m = nullptr, *pin = nullptr;
-    cudaError_t e = cudaMalloc(&m, L.total);
-    if (e == cudaSuccess) e = cudaMallocHost(&pin, L.pin);
+    cudaError_t e = cudaMalloc(&m, S.off);
+    if (e == cudaSuccess) e = cudaMallocHost(&pin, std::max(P.off, Q.off));
     if (e == cudaSuccess) {
-        pixsel_pattern((uint8_t *) pin, (size_t) c->w * c->h);
-        e = cudaMemcpy(m + L.rp, pin, (size_t) c->w * c->h, cudaMemcpyHostToDevice);
+        Arena D(m);
+        const PixselFixed f = pixsel_regions(D, c->w, c->h, true, a);
+        pixsel_pattern((uint8_t *) pin, px);
+        e = cudaMemcpy(f.rp, pin, px, cudaMemcpyHostToDevice);
     }
     if (e != cudaSuccess) {
         if (m) cudaFree(m);
@@ -786,27 +736,20 @@ static int pixsel_run(ldso_b200_ctx *c, const char *what, int slot, const ldso_b
     RET_IF(pixsel_ensure(c));
     const int w = c->w, h = c->h;
     const size_t px = (size_t) w * h;
-    const PixselLayout L = pixsel_layout(w, h);
-    char *m = c->pix_mem;
+    Arena D(c->pix_mem);
+    const PixselFixed f = pixsel_regions(D, w, h, traces, a);
     a.img0 = c->img[slot][0]; a.img1 = c->img[slot][1]; a.img2 = c->img[slot][2];
     a.B = nullptr;
     if (B) {
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(m + L.B, B, sizeof(float) * 256, cudaMemcpyHostToDevice, c->stream));
-        a.B = (const float *) (m + L.B);
+        H2D(f.B, B, sizeof(float) * 256);
+        a.B = f.B;
     }
     a.w = w; a.h = h; a.w1 = c->lw[1]; a.w2 = c->lw[2];
     a.w32 = w / 32; a.h32 = h / 32;
     a.minGradHistCut = p->minGradHistCut; a.minGradHistAdd = p->minGradHistAdd;
-    a.ths = (float *) (m + L.ths); a.thsS = (float *) (m + L.thsS);
-    a.rp = (const uint8_t *) (m + L.rp);
+    a.rp = f.rp;
     a.thFactor = p->th_factor; a.dw1 = p->gradDownweightPerLevel; a.dw2 = a.dw1 * a.dw1;
     a.dirDist = p->selectDirectionDistribution != 0;
-    a.mask = (uint16_t *) (m + L.mask); a.dir = (uint8_t *) (m + L.dir); a.map = (uint8_t *) (m + L.map);
-    a.hdr = (int *) (m + L.hdr);
-    a.rowcnt = (int *) (m + L.rowcnt); a.rowoff = (int *) (m + L.rowoff); a.list = (int *) (m + L.list);
-    a.sx = a.sy = nullptr; a.stype = nullptr; a.fu = a.fv = a.ftype = nullptr;
-    if (traces) { a.fu = (float *) (m + L.out); a.fv = a.fu + px; a.ftype = a.fv + px; }
-    else { a.sx = (int32_t *) (m + L.out); a.sy = a.sx + px; a.stype = (uint8_t *) (a.sy + px); }
     const int ncell32 = a.w32 * a.h32;
     if (ncell32 > 0) {                  // makeHists: once per call, whatever the potential
         k_pixsel_hist<<<ncell32, 1024, 0, c->stream>>>(a);
@@ -816,7 +759,10 @@ static int pixsel_run(ldso_b200_ctx *c, const char *what, int slot, const ldso_b
     }
     int pot = *current_potential, rec = p->recursions_left, ideal = pot;
     float quotia = 0.f;
-    const int *hh = (const int *) c->pix_pin;
+    PixselArgs hp;
+    Arena P(c->pix_pin);
+    pixsel_pin_regions(P, 0, px, traces, hp);
+    const int *hh = hp.hdr;
     for (;;) {
         // a potential of max(w, h) or more gives one cell, one 2pot and one 4pot block covering the image: the same pass
         const int pg = std::min(pot, std::max(w, h));
@@ -829,7 +775,7 @@ static int pixsel_run(ldso_b200_ctx *c, const char *what, int slot, const ldso_b
         LAUNCH_CHECK(c);
         k_pixsel_pick<<<(a.bw4 * a.bh4 + 127) / 128, 128, 0, c->stream>>>(a);
         LAUNCH_CHECK(c);
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(c->pix_pin, a.hdr, 16, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK_RET(c, cudaMemcpyAsync(hp.hdr, a.hdr, 16, cudaMemcpyDeviceToHost, c->stream));
         CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
         R.n2 = hh[PIXSEL_N2]; R.n3 = hh[PIXSEL_N3]; R.n4 = hh[PIXSEL_N4];
         const float numHave = (float) (R.n2 + R.n3 + R.n4), numWant = p->density;
@@ -857,7 +803,7 @@ static int pixsel_run(ldso_b200_ctx *c, const char *what, int slot, const ldso_b
     LAUNCH_CHECK(c);
     k_pixsel_finish<<<1, 1024, 0, c->stream>>>(a);
     LAUNCH_CHECK(c);
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(c->pix_pin, a.hdr, 64, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(hp.hdr, a.hdr, 4 * PIXSEL_HDR_INTS, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     R.nsel = hh[PIXSEL_NSEL]; R.nkept = hh[PIXSEL_NKEPT]; R.nfeat = hh[PIXSEL_NFEAT]; R.pot = ideal;
     return LDSO_B200_OK;
@@ -873,16 +819,18 @@ extern "C" int ldso_b200_select_pixels(ldso_b200_ctx *c, int slot, const ldso_b2
     const size_t px = (size_t) c->w * c->h;
     const int n = R.nkept;
     if (out->capacity < n) return c->fail(LDSO_B200_ERR_ARG, "select_pixels: capacity below the number of selected pixels");
-    char *q = c->pix_pin + 64;
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(q, a.sx, 4 * (size_t) n, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 4 * (size_t) n, a.sy, 4 * (size_t) n, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 8 * (size_t) n, a.stype, (size_t) n, cudaMemcpyDeviceToHost, c->stream));
-    if (out->map) CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 9 * (size_t) n, a.map, px, cudaMemcpyDeviceToHost, c->stream));
+    PixselArgs h;
+    Arena P(c->pix_pin);
+    pixsel_pin_regions(P, (size_t) n, px, false, h);
+    D2H(h.sx, a.sx, 4 * (size_t) n);
+    D2H(h.sy, a.sy, 4 * (size_t) n);
+    D2H(h.stype, a.stype, (size_t) n);
+    if (out->map) D2H(h.map, a.map, px);
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
-    memcpy(out->x, q, 4 * (size_t) n);
-    memcpy(out->y, q + 4 * (size_t) n, 4 * (size_t) n);
-    memcpy(out->type, q + 8 * (size_t) n, (size_t) n);
-    if (out->map) memcpy(out->map, q + 9 * (size_t) n, px);
+    memcpy(out->x, h.sx, 4 * (size_t) n);
+    memcpy(out->y, h.sy, 4 * (size_t) n);
+    memcpy(out->type, h.stype, (size_t) n);
+    if (out->map) memcpy(out->map, h.map, px);
     out->n = n; out->n2 = R.n2; out->n3 = R.n3; out->n4 = R.n4;
     *current_potential = R.pot;
     return LDSO_B200_OK;
@@ -920,32 +868,29 @@ static int dev_upload(ldso_b200_ctx *c, T *dst, const T *src, size_t count) {
 //    ^ uploaded only when the CSR changes         ^---- upload range ------^
 //                                                 ^----------- download range (one D2H) ----------^
 // so a set_window is one pack + one cudaMemcpyAsync + one memset, and reading points/residuals back is one copy.
-struct Arena {
-    size_t off = 0;
-    size_t take(size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t) 255; return o; }
-};
-
 static int alloc_window(ldso_b200_ctx *c, int nP, int nR) {
     DevWindow &d = c->d;
     Arena A;
+    // every region starts and ends on a 256-byte boundary, so the range ends below (topo_end, ...) are region starts as well
+    auto take = [&](size_t bytes) { return (size_t) A.take((bytes + 255) & ~(size_t) 255, 256); };
     const size_t nPs = std::max(nP, 32), nRs = std::max(nR, 32);
     auto &L = c->lay;
-    L.pt_host = A.take(4 * nPs); L.pt_res_begin = A.take(4 * (nPs + 1)); L.res_point = A.take(4 * nRs); L.res_target = A.take(4 * nRs);
+    L.pt_host = take(4 * nPs); L.pt_res_begin = take(4 * (nPs + 1)); L.res_point = take(4 * nRs); L.res_target = take(4 * nRs);
     L.topo_end = A.off;
-    L.pt_u = A.take(4 * nPs); L.pt_v = A.take(4 * nPs); L.pt_color = A.take(32 * nPs); L.pt_weights = A.take(32 * nPs);
-    L.pt_priorF = A.take(4 * nPs); L.pt_idepth_backup = A.take(4 * nPs); L.res_lin = A.take(nRs);
-    L.res_state = A.take(nRs);
+    L.pt_u = take(4 * nPs); L.pt_v = take(4 * nPs); L.pt_color = take(32 * nPs); L.pt_weights = take(32 * nPs);
+    L.pt_priorF = take(4 * nPs); L.pt_idepth_backup = take(4 * nPs); L.res_lin = take(nRs);
+    L.res_state = take(nRs);
     L.dl_begin = A.off;
-    L.pt_idepth = A.take(4 * nPs); L.pt_idepth_zero = A.take(4 * nPs);
+    L.pt_idepth = take(4 * nPs); L.pt_idepth_zero = take(4 * nPs);
     L.ul_end = A.off;
-    L.pt_step = A.take(4 * nPs); L.pt_HdiF = A.take(4 * nPs); L.pt_bdSumF = A.take(4 * nPs); L.pt_Hdd = A.take(4 * nPs);
-    L.pt_bd = A.take(4 * nPs); L.pt_Hcd = A.take(16 * nPs);
-    L.res_new_state = A.take(nRs); L.res_active = A.take(nRs); L.res_energy = A.take(4 * nRs); L.res_new_energy = A.take(4 * nRs);
-    L.res_new_energy_wo = A.take(4 * nRs);
+    L.pt_step = take(4 * nPs); L.pt_HdiF = take(4 * nPs); L.pt_bdSumF = take(4 * nPs); L.pt_Hdd = take(4 * nPs);
+    L.pt_bd = take(4 * nPs); L.pt_Hcd = take(16 * nPs);
+    L.res_new_state = take(nRs); L.res_active = take(nRs); L.res_energy = take(4 * nRs); L.res_new_energy = take(4 * nRs);
+    L.res_new_energy_wo = take(4 * nRs);
     L.dl_light_end = A.off;
-    L.res_JpJdF = A.take(32 * nRs);
+    L.res_JpJdF = take(32 * nRs);
     L.dl_end = A.off;
-    L.res_JpJdF_new = A.take(32 * nRs);
+    L.res_JpJdF_new = take(32 * nRs);
     L.total = A.off;
     // res_state is both an input and a result: it sits right before dl_begin and is fetched separately (tiny)
     CUDA_CHECK_RET(c, cudaMalloc(&c->arena_dev, L.total));
@@ -1380,7 +1325,25 @@ static int clear_select(ldso_b200_ctx *c) {   // multi-GPU: slots owned by other
     return LDSO_B200_OK;
 }
 
-static int trace_reserve(ldso_b200_ctx *c, size_t bytes);      // device scratch shared by the one-shot entry points
+// grows a one-shot scratch block, device or pinned, to at least `bytes`; what it held is not kept
+static int scratch_reserve(ldso_b200_ctx *c, char *&buf, size_t &cap, size_t bytes, bool pinned) {
+    if (bytes <= cap) return LDSO_B200_OK;
+    if (buf) { if (pinned) cudaFreeHost(buf); else cudaFree(buf); }
+    buf = nullptr; cap = 0;
+    CUDA_CHECK_RET(c, pinned ? cudaMallocHost(&buf, bytes) : cudaMalloc(&buf, bytes));
+    cap = bytes;
+    return LDSO_B200_OK;
+}
+// sizes one call's device scratch with its region list (scratch_layout.cuh), grows trace_buf to fit, and carves it with the same list
+template <typename List>
+static int trace_carve(ldso_b200_ctx *c, List &&list) {
+    Arena S;
+    list(S);
+    RET_IF(scratch_reserve(c, c->trace_buf, c->trace_cap, S.off, false));
+    Arena D(c->trace_buf);
+    list(D);
+    return LDSO_B200_OK;
+}
 static int flush_select(ldso_b200_ctx *c);                      // run a deferred setNewFrameEnergyTH select (fused loop)
 extern "C" int ldso_b200_linearize_all(ldso_b200_ctx *c, int fixLinearization, int flags, double *energy_out) {
     if (!c) return LDSO_B200_ERR_ARG;
@@ -1568,14 +1531,13 @@ extern "C" int ldso_b200_calc_energies(ldso_b200_ctx *c, double *energyL, double
     RET_IF(build_derived(c));
     if (c->prior_dim != 0 && c->prior_dim != c->n) return c->fail(LDSO_B200_ERR_STATE, "prior dimension does not match the frames: call set_frames first");
     const int nb = std::max(1, (c->d.nP + KEN_THREADS - 1) / KEN_THREADS);
-    RET_IF(trace_reserve(c, sizeof(double) * ((size_t) nb + 4) + 16));
-    double *part = (double *) c->trace_buf, *out = part + nb;
-    unsigned *counter = (unsigned *) (out + 2);
-    CUDA_CHECK_RET(c, cudaMemsetAsync(counter, 0, sizeof(unsigned), c->stream));
-    k_calc_energies<<<nb, KEN_THREADS, 0, c->stream>>>(c->d, c->ws_dev, c->sb, part, counter, out);
+    EnergyScratch E;
+    RET_IF(trace_carve(c, [&](Arena &A) { calc_energies_regions(A, nb, E); }));
+    CUDA_CHECK_RET(c, cudaMemsetAsync(E.counter, 0, sizeof(unsigned), c->stream));
+    k_calc_energies<<<nb, KEN_THREADS, 0, c->stream>>>(c->d, c->ws_dev, c->sb, E.part, E.counter, E.out);
     LAUNCH_CHECK(c);
     double h[2];
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(h, out, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(h, E.out, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     if (energyL) *energyL = h[0];
     if (energyM) *energyM = h[1];
@@ -1612,14 +1574,6 @@ static TraceSettingsDev trace_settings(const ldso_b200_ctx *c) {
     T.trace_minImprovementFactor = c->S.trace_minImprovementFactor;
     return T;
 }
-static int trace_reserve(ldso_b200_ctx *c, size_t bytes) {
-    if (bytes <= c->trace_cap) return LDSO_B200_OK;
-    if (c->trace_buf) cudaFree(c->trace_buf);
-    c->trace_buf = nullptr; c->trace_cap = 0;
-    CUDA_CHECK_RET(c, cudaMalloc(&c->trace_buf, bytes));
-    c->trace_cap = bytes;
-    return LDSO_B200_OK;
-}
 
 extern "C" int ldso_b200_immature_init(ldso_b200_ctx *c, int host_slot, int n, const float *u, const float *v, float *color8,
                                        float *weights8, float *gradH4, float *energyTH) {
@@ -1628,14 +1582,14 @@ extern "C" int ldso_b200_immature_init(ldso_b200_ctx *c, int host_slot, int n, c
     if (n == 0) return LDSO_B200_OK;
     cudaSetDevice(c->device);
     const size_t N = (size_t) n;
-    RET_IF(trace_reserve(c, sizeof(float) * N * 23));
-    float *du = (float *) c->trace_buf, *dv = du + N, *dc = dv + N, *dw = dc + 8 * N, *dg = dw + 8 * N, *de = dg + 4 * N;
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(du, u, 4 * N, cudaMemcpyHostToDevice, c->stream));
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(dv, v, 4 * N, cudaMemcpyHostToDevice, c->stream));
-    CUDA_CHECK_RET(c, cudaMemsetAsync(dc, 0, sizeof(float) * N * 21, c->stream));
-    launch_immature_init(n, c->img[host_slot][0], c->w, du, dv, trace_settings(c), dc, dw, dg, de, c->stream);
+    ImmInitScratch s;
+    RET_IF(trace_carve(c, [&](Arena &A) { immature_init_regions(A, N, s); }));
+    H2D(s.u, u, 4 * N);
+    H2D(s.v, v, 4 * N);
+    CUDA_CHECK_RET(c, cudaMemsetAsync(s.color8, 0, sizeof(float) * N * 21, c->stream));      // the outputs' region
+    launch_immature_init(n, c->img[host_slot][0], c->w, s.u, s.v, trace_settings(c), s.color8, s.weights8, s.gradH4, s.energyTH, c->stream);
     LAUNCH_CHECK(c);
-    D2H(color8, dc, 32 * N); D2H(weights8, dw, 32 * N); D2H(gradH4, dg, 16 * N); D2H(energyTH, de, 4 * N);
+    D2H(color8, s.color8, 32 * N); D2H(weights8, s.weights8, 32 * N); D2H(gradH4, s.gradH4, 16 * N); D2H(energyTH, s.energyTH, 4 * N);
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     return LDSO_B200_OK;
 }
@@ -1652,30 +1606,18 @@ extern "C" int ldso_b200_trace_immature(ldso_b200_ctx *c, int new_slot, const ld
     for (int i = 0; i < n; i++) if (p->host[i] < 0 || p->host[i] >= n_hosts) return c->fail(LDSO_B200_ERR_ARG, "candidate host index out of range");
     cudaSetDevice(c->device);
     const size_t N = (size_t) n, H = (size_t) n_hosts;
-    // layout (floats): u v color8 weights8 gradH4 energyTH | idmin idmax quality uv2 interval | host status (ints) | KRKi Kt aff
-    const size_t nf = N * (2 + 8 + 8 + 4 + 1) + N * (3 + 2 + 1) + 2 * N + H * 14;
-    RET_IF(trace_reserve(c, sizeof(float) * nf));
-    float *q = (float *) c->trace_buf;
     TraceArgs A;
+    RET_IF(trace_carve(c, [&](Arena &R) { trace_immature_regions(R, N, H, A); }));
     A.n = n; A.w = c->w; A.h = c->h; A.img = c->img[new_slot][0]; A.S = trace_settings(c);
-    float *du = q; q += N; float *dv = q; q += N; float *dc = q; q += 8 * N; float *dw = q; q += 8 * N; float *dg = q; q += 4 * N; float *de = q; q += N;
-    float *dmin = q; q += N; float *dmax = q; q += N; float *dq = q; q += N; float *duv = q; q += 2 * N; float *div = q; q += N;
-    int *dh = (int *) q; q += N; int *ds = (int *) q; q += N;
-    float *dK = q; q += 9 * H; float *dt = q; q += 3 * H; float *da = q; q += 2 * H;
-#define TR_H2D(dst, src, bytes) CUDA_CHECK_RET(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, c->stream))
-    TR_H2D(du, p->u, 4 * N); TR_H2D(dv, p->v, 4 * N); TR_H2D(dc, p->color8, 32 * N); TR_H2D(dw, p->weights8, 32 * N);
-    TR_H2D(dg, p->gradH4, 16 * N); TR_H2D(de, p->energyTH, 4 * N); TR_H2D(dmin, p->idepth_min, 4 * N); TR_H2D(dmax, p->idepth_max, 4 * N);
-    TR_H2D(dq, p->quality, 4 * N); TR_H2D(duv, p->lastTraceUV2, 8 * N); TR_H2D(div, p->lastTracePixelInterval, 4 * N);
-    TR_H2D(dh, p->host, 4 * N); TR_H2D(ds, p->lastTraceStatus, 4 * N);
-    TR_H2D(dK, KRKi9, 36 * H); TR_H2D(dt, Kt3, 12 * H); TR_H2D(da, aff2, 8 * H);
-#undef TR_H2D
-    A.u = du; A.v = dv; A.color8 = dc; A.weights8 = dw; A.gradH4 = dg; A.energyTH = de; A.host = dh;
-    A.KRKi9 = dK; A.Kt3 = dt; A.aff2 = da;
-    A.idepth_min = dmin; A.idepth_max = dmax; A.quality = dq; A.status = ds; A.uv2 = duv; A.interval = div;
+    H2D(A.u, p->u, 4 * N); H2D(A.v, p->v, 4 * N); H2D(A.color8, p->color8, 32 * N); H2D(A.weights8, p->weights8, 32 * N);
+    H2D(A.gradH4, p->gradH4, 16 * N); H2D(A.energyTH, p->energyTH, 4 * N); H2D(A.idepth_min, p->idepth_min, 4 * N); H2D(A.idepth_max, p->idepth_max, 4 * N);
+    H2D(A.quality, p->quality, 4 * N); H2D(A.uv2, p->lastTraceUV2, 8 * N); H2D(A.interval, p->lastTracePixelInterval, 4 * N);
+    H2D(A.host, p->host, 4 * N); H2D(A.status, p->lastTraceStatus, 4 * N);
+    H2D(A.KRKi9, KRKi9, 36 * H); H2D(A.Kt3, Kt3, 12 * H); H2D(A.aff2, aff2, 8 * H);
     launch_trace_on(A, c->stream);
     LAUNCH_CHECK(c);
-    D2H(p->idepth_min, dmin, 4 * N); D2H(p->idepth_max, dmax, 4 * N); D2H(p->quality, dq, 4 * N); D2H(p->lastTraceStatus, ds, 4 * N);
-    D2H(p->lastTraceUV2, duv, 8 * N); D2H(p->lastTracePixelInterval, div, 4 * N);
+    D2H(p->idepth_min, A.idepth_min, 4 * N); D2H(p->idepth_max, A.idepth_max, 4 * N); D2H(p->quality, A.quality, 4 * N); D2H(p->lastTraceStatus, A.status, 4 * N);
+    D2H(p->lastTraceUV2, A.uv2, 8 * N); D2H(p->lastTracePixelInterval, A.interval, 4 * N);
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     return LDSO_B200_OK;
 }
@@ -1693,18 +1635,14 @@ extern "C" int ldso_b200_optimize_immature(ldso_b200_ctx *c, int n, const float 
     for (int i = 0; i < n; i++) if (host[i] < 0 || host[i] >= nF) return c->fail(LDSO_B200_ERR_ARG, "candidate host index out of range");
     cudaSetDevice(c->device);
     const size_t N = (size_t) n;
-    const size_t nf = N * (2 + 2 + 8 + 8 + 1) + N /*host*/ + N /*ok*/ + N /*idepth*/ + (N * nF + 3) / 4 + 4;
-    RET_IF(trace_reserve(c, sizeof(float) * nf));
-    float *q = (float *) c->trace_buf;
-    float *du = q; q += N; float *dv = q; q += N; float *dmin = q; q += N; float *dmax = q; q += N; float *dc = q; q += 8 * N; float *dw = q; q += 8 * N;
-    float *de = q; q += N; int *dh = (int *) q; q += N; int *dok = (int *) q; q += N; float *did = q; q += N; unsigned char *dst = (unsigned char *) q;
-#define TR_H2D(dst_, src_, bytes_) CUDA_CHECK_RET(c, cudaMemcpyAsync(dst_, src_, bytes_, cudaMemcpyHostToDevice, c->stream))
-    TR_H2D(du, u, 4 * N); TR_H2D(dv, v, 4 * N); TR_H2D(dmin, idepth_min, 4 * N); TR_H2D(dmax, idepth_max, 4 * N); TR_H2D(dc, color8, 32 * N);
-    TR_H2D(dw, weights8, 32 * N); TR_H2D(de, energyTH, 4 * N); TR_H2D(dh, host, 4 * N);
-#undef TR_H2D
-    launch_optimize_immature(n, c->ws_dev, du, dv, dh, dmin, dmax, dc, dw, de, min_obs, dok, did, dst, c->stream);
+    OptImmScratch s;
+    RET_IF(trace_carve(c, [&](Arena &A) { optimize_immature_regions(A, N, nF, s); }));
+    H2D(s.u, u, 4 * N); H2D(s.v, v, 4 * N); H2D(s.idmin, idepth_min, 4 * N); H2D(s.idmax, idepth_max, 4 * N); H2D(s.color8, color8, 32 * N);
+    H2D(s.weights8, weights8, 32 * N); H2D(s.energyTH, energyTH, 4 * N); H2D(s.host, host, 4 * N);
+    launch_optimize_immature(n, c->ws_dev, s.u, s.v, s.host, s.idmin, s.idmax, s.color8, s.weights8, s.energyTH, min_obs, s.ok, s.idepth, s.res_state,
+                             c->stream);
     LAUNCH_CHECK(c);
-    D2H(ok, dok, 4 * N); D2H(idepth, did, 4 * N); D2H(res_state, dst, N * nF);
+    D2H(ok, s.ok, 4 * N); D2H(idepth, s.idepth, 4 * N); D2H(res_state, s.res_state, N * nF);
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     return LDSO_B200_OK;
 }
@@ -1726,52 +1664,39 @@ extern "C" int ldso_b200_select_activation(ldso_b200_ctx *c, int newest_frame, f
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
     const int w1 = c->w >> 1, h1 = c->h >> 1;
-    const size_t N = (size_t) std::max(n, 1), cells = (size_t) w1 * h1, map_bytes = (cells + 3) & ~(size_t) 3;
-    // layout of the scratch buffer (4-byte units first, bytes last)
-    const size_t words = 2 * cells /*frontiers*/ + 12 * N /*7 float + 2 int inputs, 3 scratch*/;
-    RET_IF(trace_reserve(c, 4 * words + map_bytes + N + MAXF + 64));
-    int *q = (int *) c->trace_buf;
+    const size_t N = (size_t) std::max(n, 1), cells = (size_t) w1 * h1;
     ActSelArgs A;
+    RET_IF(trace_carve(c, [&](Arena &R) { actsel_regions(R, c->w, c->h, N, A); }));
+    const size_t map_bytes = A.map_bytes;
     A.ws = c->ws_dev; A.newest = newest_frame; A.w1 = w1; A.h1 = h1;
     A.nP = c->d.nP; A.pt_host = c->d.pt_host; A.pt_u = c->d.pt_u; A.pt_v = c->d.pt_v; A.pt_idepth = c->d.pt_idepth;
     A.n = n;
-    A.front0 = q; q += cells; A.front1 = q; q += cells;
-    float *du = (float *) q; q += N; float *dv = (float *) q; q += N; float *dmin = (float *) q; q += N; float *dmax = (float *) q; q += N;
-    float *dq = (float *) q; q += N; float *di = (float *) q; q += N; float *dt = (float *) q; q += N; int *ds = q; q += N; int *dh = q; q += N;
-    A.pre_idx = q; q += N; A.pre_frac = (float *) q; q += N; A.pre_thresh = (float *) q; q += N;
-    unsigned char *b = (unsigned char *) q;
-    A.map = b; b += map_bytes; A.action = b; b += N; unsigned char *dflag = b;
-    A.map_bytes = (int) map_bytes;
-    A.u = du; A.v = dv; A.idmin = dmin; A.idmax = dmax; A.quality = dq; A.interval = di; A.my_type = dt; A.status = ds; A.host = dh; A.flagged = dflag;
     A.currentMinActDist = current_min_act_dist; A.minTraceQuality = min_trace_quality;
     // the kernel also has a global-memory map path (use_smem = 0) for larger images; it has not been exercised on hardware yet, so
     // larger images are refused rather than served by an unvalidated path (level 1 of 1240x376 needs 114 KB)
     if (map_bytes > 200 * 1024) return c->fail(LDSO_B200_ERR_ARG, "select_activation: level-1 image larger than 200 KB (one byte per pixel must fit in shared memory)");
     A.use_smem = 1;
-    // the nine candidate arrays and the frame flags travel as ONE pinned staging block laid out like the device block
-    const size_t in_words = 9 * N, in_bytes = 4 * in_words, stage_bytes = in_bytes + N + MAXF + 16;
-    if (stage_bytes > c->actsel_pin_cap) {
-        if (c->actsel_pin) cudaFreeHost(c->actsel_pin);
-        c->actsel_pin = nullptr; c->actsel_pin_cap = 0;
-        CUDA_CHECK_RET(c, cudaHostAlloc((void **) &c->actsel_pin, stage_bytes * 2, cudaHostAllocDefault));
-        c->actsel_pin_cap = stage_bytes * 2;
-    }
+    // the candidates and the frame flags travel through a pinned stage laid out like the device's inputs (actsel_inputs)
+    ActSelArgs S;
+    Arena P;
+    actsel_stage_regions(P, N, S);
+    RET_IF(scratch_reserve(c, c->actsel_pin, c->actsel_pin_cap, P.off, true));
+    P = Arena(c->actsel_pin);
+    actsel_stage_regions(P, N, S);
     {
-        unsigned char *hp = c->actsel_pin;
-        const void *src[9] = {u, v, idepth_min, idepth_max, quality, lastTracePixelInterval, my_type, lastTraceStatus, host};
-        for (int k = 0; k < 9; k++) if (n > 0) memcpy(hp + 4 * N * k, src[k], 4 * (size_t) n);
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(du, hp, in_bytes, cudaMemcpyHostToDevice, c->stream));      // du .. dh are contiguous
-        memcpy(hp + in_bytes, frame_flagged, (size_t) nF);
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(dflag, hp + in_bytes, (size_t) nF, cudaMemcpyHostToDevice, c->stream));
+        const struct { const void *dst, *src; } in[] = {{S.u, u}, {S.v, v}, {S.idmin, idepth_min}, {S.idmax, idepth_max}, {S.quality, quality},
+                                                        {S.interval, lastTracePixelInterval}, {S.my_type, my_type}, {S.status, lastTraceStatus}, {S.host, host}};
+        if (n > 0) for (const auto &x : in) memcpy((void *) x.dst, x.src, 4 * (size_t) n);
+        H2D(A.u, S.u, 36 * N);      // the nine arrays are one region
+        memcpy((void *) S.flagged, frame_flagged, (size_t) nF);
+        H2D(A.flagged, S.flagged, (size_t) nF);
     }
-    A.dbg = c->ktime ? (long long *) (dflag + MAXF) : nullptr;      // 8-byte aligned below
-    if (A.dbg) A.dbg = (long long *) (((uintptr_t) A.dbg + 7) & ~(uintptr_t) 7);
+    if (!c->ktime) A.dbg = nullptr;
     c->kt_begin("actsel");
     launch_activation_select(A, c->stream);
     c->kt_end();
     LAUNCH_CHECK(c);
-    unsigned char *hact = c->actsel_pin + in_bytes + MAXF + 8;
-    if (n > 0) D2H(hact, A.action, (size_t) n);
+    if (n > 0) D2H(S.action, A.action, (size_t) n);
     if (dist_map) {
         c->h_scratch_bytes.resize(map_bytes);
         D2H(c->h_scratch_bytes.data(), A.map, map_bytes);
@@ -1779,7 +1704,7 @@ extern "C" int ldso_b200_select_activation(ldso_b200_ctx *c, int newest_frame, f
     long long stamps[4] = {0, 0, 0, 0};
     if (A.dbg) D2H(stamps, A.dbg, sizeof(stamps));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
-    if (n > 0) memcpy(action, hact, (size_t) n);
+    if (n > 0) memcpy(action, S.action, (size_t) n);
     if (A.dbg) fprintf(stderr, "[ldso_b200 actsel] cycles: map+seeds+grow %lld, candidate terms %lld, sequential pass %lld\n", stamps[1] - stamps[0],
                        stamps[2] - stamps[1], stamps[3] - stamps[2]);
     if (dist_map) for (size_t i = 0; i < cells; i++) dist_map[i] = c->h_scratch_bytes[i] == 255 ? 1000.f : (float) c->h_scratch_bytes[i];   // fwdWarpedIDDistFinal's values
@@ -1787,25 +1712,6 @@ extern "C" int ldso_b200_select_activation(ldso_b200_ctx *c, int newest_frame, f
 }
 
 // ---------------------------------------------------------------------------------------------- immature-point store
-// activate_immature's device scratch (sized for every candidate of a full window: (MAXF-1) segments) and the pinned block, whose
-// first 64 bytes hold the header, traceNewCoarse's counters and the frame flags, and the rest a segment or the released records
-// scratch: 38 words per candidate (gathered, k_activation_select's terms, selected, LM results), res_state and action bytes, the two
-// BFS frontiers, the distance map, 64 bytes of flags / header / counters, the released records
-struct ImmLayout { size_t maxc, cells, map_bytes, bytes, front, map, small, rec, scratch, pin; };
-static ImmLayout imm_layout(const ldso_b200_ctx *c, int cap) {
-    ImmLayout L;
-    L.maxc = (size_t) (MAXF - 1) * cap;
-    L.cells = (size_t) (c->w >> 1) * (c->h >> 1);
-    L.map_bytes = (L.cells + 3) & ~(size_t) 3;
-    L.bytes = align16(L.maxc * 4 * 38);
-    L.front = L.bytes + align16(L.maxc * (MAXF + 1));
-    L.map = L.front + align16(8 * L.cells);
-    L.small = L.map + align16(L.map_bytes);
-    L.rec = L.small + 64;
-    L.scratch = L.rec + L.maxc * sizeof(ImmRecord);
-    L.pin = 64 + std::max((size_t) IMM_SEG_WORDS * 4 * cap, L.maxc * sizeof(ImmRecord));
-    return L;
-}
 static cudaError_t imm_copy_segment(const ImmSeg &d, const ImmSeg &s, size_t n, cudaStream_t st) {
     const struct { void *dst; const void *src; size_t words; } f[] = {
         {d.u, s.u, 1}, {d.v, s.v, 1}, {d.my_type, s.my_type, 1}, {d.color8, s.color8, 8}, {d.weights8, s.weights8, 8}, {d.gradH4, s.gradH4, 4},
@@ -1823,12 +1729,16 @@ static cudaError_t imm_copy_segment(const ImmSeg &d, const ImmSeg &s, size_t n, 
 // grows the store to at least cap entries per segment; every segment keeps its entries (live or released), copied to the new stride
 static int imm_reserve(ldso_b200_ctx *c, int cap) {
     if (cap <= c->imm_cap) return LDSO_B200_OK;
-    const ImmLayout L = imm_layout(c, cap);
+    StoreActArgs P;
+    ActSelArgs A;
+    Arena S, H;
+    imm_scratch_regions(S, cap, c->w, c->h, P, A);
+    imm_pin_regions(H, cap);
     float *store = nullptr;
     char *scratch = nullptr, *pin = nullptr;
     cudaError_t e = cudaMalloc(&store, sizeof(float) * IMM_SEG_WORDS * (size_t) cap * NSLOTS);
-    if (e == cudaSuccess) e = cudaMalloc(&scratch, L.scratch);
-    if (e == cudaSuccess) e = cudaMallocHost(&pin, L.pin);
+    if (e == cudaSuccess) e = cudaMalloc(&scratch, S.off);
+    if (e == cudaSuccess) e = cudaMallocHost(&pin, H.off);
     for (int s = 0; s < NSLOTS && e == cudaSuccess; s++)
         if (c->imm_n[s] > 0) e = imm_copy_segment(imm_seg(store, cap, s), imm_seg(c->imm_store, c->imm_cap, s), (size_t) c->imm_n[s], c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -1883,7 +1793,8 @@ extern "C" int ldso_b200_immature_seed(ldso_b200_ctx *c, int slot, int n, const 
     c->imm_n[slot] = 0;
     if (n == 0) return LDSO_B200_OK;
     const ImmSeg g = imm_seg(c->imm_store, c->imm_cap, slot);
-    float *hp = (float *) (c->imm_pin + 64);
+    Arena H(c->imm_pin);
+    float *hp = (float *) imm_pin_regions(H, c->imm_cap).body;      // u, v, my_type: n each
     const size_t N = (size_t) n;
     memcpy(hp, u, 4 * N); memcpy(hp + N, v, 4 * N);
     if (my_type) memcpy(hp + 2 * N, my_type, 4 * N);
@@ -1918,17 +1829,19 @@ extern "C" int ldso_b200_make_new_traces_pixels(ldso_b200_ctx *c, int slot, cons
         launch_store_compact(c->imm_store, c->imm_cap, slot, nf, a.hdr + PIXSEL_NSEED, c->stream);
         LAUNCH_CHECK(c);
         const ImmSeg g = imm_seg(c->imm_store, c->imm_cap, slot);
-        char *q = c->pix_pin;
         const size_t N = (size_t) nf;
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(q, a.hdr, 64, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 64, g.u, 4 * N, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 64 + 4 * N, g.v, 4 * N, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK_RET(c, cudaMemcpyAsync(q + 64 + 8 * N, g.my_type, 4 * N, cudaMemcpyDeviceToHost, c->stream));
+        PixselArgs h;
+        Arena P(c->pix_pin);
+        pixsel_pin_regions(P, N, (size_t) c->w * c->h, true, h);
+        D2H(h.hdr, a.hdr, 4 * PIXSEL_HDR_INTS);
+        D2H(h.fu, g.u, 4 * N);
+        D2H(h.fv, g.v, 4 * N);
+        D2H(h.ftype, g.my_type, 4 * N);
         CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
-        n = ((const int *) q)[PIXSEL_NSEED];
-        memcpy(out->u, q + 64, 4 * (size_t) n);
-        memcpy(out->v, q + 64 + 4 * N, 4 * (size_t) n);
-        memcpy(out->my_type, q + 64 + 8 * N, 4 * (size_t) n);
+        n = h.hdr[PIXSEL_NSEED];
+        memcpy(out->u, h.fu, 4 * (size_t) n);
+        memcpy(out->v, h.fv, 4 * (size_t) n);
+        memcpy(out->my_type, h.ftype, 4 * (size_t) n);
     }
     c->imm_n[slot] = c->imm_live[slot] = n;
     out->n_selected = R.nkept; out->n = n;
@@ -1960,13 +1873,16 @@ extern "C" int ldso_b200_trace_new_coarse(ldso_b200_ctx *c, int new_slot, int n_
     memset(&P.T, 0, sizeof(P.T));
     P.T.w = c->w; P.T.h = c->h; P.T.img = c->img[new_slot][0]; P.T.S = trace_settings(c);
     P.store = c->imm_store; P.cap = c->imm_cap;
-    const ImmLayout L = imm_layout(c, c->imm_cap);
-    P.counts = counts7 ? (int *) (c->imm_scratch + L.small + 32) : nullptr;
+    StoreActArgs act;      // activate_immature's regions: only the counters are used here
+    ActSelArgs sel;
+    Arena D(c->imm_scratch), H(c->imm_pin);
+    const ImmSmall small = imm_scratch_regions(D, c->imm_cap, c->w, c->h, act, sel);
+    P.counts = counts7 ? small.counts : nullptr;
     if (P.counts) CUDA_CHECK_RET(c, cudaMemsetAsync(P.counts, 0, sizeof(int) * 7, c->stream));
     launch_store_trace(P, c->stream);
     LAUNCH_CHECK(c);
     if (counts7) {
-        int *hc = (int *) (c->imm_pin + 16);
+        int *hc = imm_pin_regions(H, c->imm_cap).small.counts;
         CUDA_CHECK_RET(c, cudaMemcpyAsync(hc, P.counts, sizeof(int) * 7, cudaMemcpyDeviceToHost, c->stream));
         CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
         memcpy(counts7, hc, sizeof(int32_t) * 7);
@@ -1999,36 +1915,23 @@ extern "C" int ldso_b200_activate_immature(ldso_b200_ctx *c, float current_min_a
     if (ncand == 0) return LDSO_B200_OK;
     cudaSetDevice(c->device);
     RET_IF(build_derived(c));
-    const ImmLayout L = imm_layout(c, c->imm_cap);
-    const size_t M = L.maxc;
     P.store = c->imm_store; P.cap = c->imm_cap; P.n = ncand; P.nF = nF; P.ws = c->ws_dev;
-    float *f32 = (float *) c->imm_scratch;
-    P.c_u = f32; P.c_v = f32 + M; P.c_idmin = f32 + 2 * M; P.c_idmax = f32 + 3 * M; P.c_quality = f32 + 4 * M; P.c_interval = f32 + 5 * M;
-    P.c_type = f32 + 6 * M;
-    P.c_status = (int *) (f32 + 7 * M); P.c_host = (int *) (f32 + 8 * M); P.c_index = (int *) (f32 + 9 * M); P.c_sel = (int *) (f32 + 10 * M);
     ActSelArgs A;
-    A.pre_idx = (int *) (f32 + 11 * M); A.pre_frac = f32 + 12 * M; A.pre_thresh = f32 + 13 * M;
-    P.s_u = f32 + 14 * M; P.s_v = f32 + 15 * M; P.s_idmin = f32 + 16 * M; P.s_idmax = f32 + 17 * M; P.s_energyTH = f32 + 18 * M;
-    P.s_idepth = f32 + 19 * M; P.s_host = (int *) (f32 + 20 * M); P.s_ok = (int *) (f32 + 21 * M);
-    P.s_color8 = f32 + 22 * M; P.s_weights8 = f32 + 30 * M;
-    P.s_res = (unsigned char *) (c->imm_scratch + L.bytes); P.action = P.s_res + M * MAXF;
-    A.front0 = (int *) (c->imm_scratch + L.front); A.front1 = A.front0 + cells;
-    A.map = (unsigned char *) (c->imm_scratch + L.map);
-    unsigned char *dflag = (unsigned char *) (c->imm_scratch + L.small);
-    P.hdr = (int *) (c->imm_scratch + L.small + 16);
-    P.rec = (ImmRecord *) (c->imm_scratch + L.rec);
+    Arena D(c->imm_scratch), H(c->imm_pin);
+    imm_scratch_regions(D, c->imm_cap, c->w, c->h, P, A);
+    const ImmPin pin = imm_pin_regions(H, c->imm_cap);
     // candidates, selection, activation LM, bookkeeping
     launch_store_gather(P, c->stream);
     LAUNCH_CHECK(c);
-    memcpy(c->imm_pin + 48, frame_flagged, (size_t) nF);
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(dflag, c->imm_pin + 48, (size_t) nF, cudaMemcpyHostToDevice, c->stream));
+    memcpy(pin.small.flags, frame_flagged, (size_t) nF);
+    H2D(A.flagged, pin.small.flags, (size_t) nF);
     A.ws = c->ws_dev; A.newest = nF - 1; A.w1 = w1; A.h1 = h1;
     A.nP = c->d.nP; A.pt_host = c->d.pt_host; A.pt_u = c->d.pt_u; A.pt_v = c->d.pt_v; A.pt_idepth = c->d.pt_idepth;
     A.n = ncand;
     A.u = P.c_u; A.v = P.c_v; A.idmin = P.c_idmin; A.idmax = P.c_idmax; A.quality = P.c_quality; A.interval = P.c_interval; A.my_type = P.c_type;
-    A.status = P.c_status; A.host = P.c_host; A.flagged = dflag;
+    A.status = P.c_status; A.host = P.c_host;
     A.currentMinActDist = current_min_act_dist; A.minTraceQuality = min_trace_quality;
-    A.action = P.action; A.map_bytes = (int) map_bytes; A.use_smem = 1; A.dbg = nullptr;
+    A.action = P.action; A.use_smem = 1; A.dbg = nullptr;
     launch_activation_select(A, c->stream);
     LAUNCH_CHECK(c);
     launch_store_pick(P, c->stream);
@@ -2037,11 +1940,11 @@ extern "C" int ldso_b200_activate_immature(ldso_b200_ctx *c, float current_min_a
     LAUNCH_CHECK(c);
     launch_store_apply(P, c->stream);
     LAUNCH_CHECK(c);
-    int *hh = (int *) c->imm_pin;
+    int *hh = pin.small.hdr;
     CUDA_CHECK_RET(c, cudaMemcpyAsync(hh, P.hdr, sizeof(int) * 4, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     const int nrel = hh[1], nvalid = hh[2];
-    const ImmRecord *hr = (const ImmRecord *) (c->imm_pin + 64);
+    const ImmRecord *hr = (const ImmRecord *) pin.body;
     if (nrel > 0) {
         CUDA_CHECK_RET(c, cudaMemcpyAsync((void *) hr, P.rec, sizeof(ImmRecord) * nrel, cudaMemcpyDeviceToHost, c->stream));
         CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
@@ -2085,7 +1988,8 @@ extern "C" int ldso_b200_immature_read(ldso_b200_ctx *c, int slot, ldso_b200_imm
     if (n == 0) return LDSO_B200_OK;
     cudaSetDevice(c->device);
     const size_t cap = c->imm_cap, N = n;
-    float *hp = (float *) (c->imm_pin + 64);
+    Arena H(c->imm_pin);
+    float *hp = (float *) imm_pin_regions(H, c->imm_cap).body;
     CUDA_CHECK_RET(c, cudaMemcpyAsync(hp, imm_seg(c->imm_store, c->imm_cap, slot).u, sizeof(float) * IMM_SEG_WORDS * cap, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     const ImmSeg g = imm_seg(hp, c->imm_cap, 0);      // the segment's layout, at the staging copy
@@ -2145,29 +2049,17 @@ extern "C" int ldso_b200_init_calc_res(ldso_b200_ctx *c, int first_slot, int new
     if (alphaEnergy > alphaK * n) { alphaOpt = 0; alphaEnergy = alphaK * n; } else alphaOpt = alphaW;
     A.alphaOpt = alphaOpt; A.couplingWeight = couplingWeight;
     const size_t N = (size_t) n, grid = (N + INIT_THREADS / 8 - 1) / (INIT_THREADS / 8);
-    const size_t words = N * (1 + 1 + 1 + 1 + 2 + 1) /*in*/ + N * (2 + 1 + 1 + 10) /*out*/ + grid * INIT_NACC + 4 + 2 * INIT_NACC + 8;
-    RET_IF(trace_reserve(c, 4 * words + 2 * N + 64));
-    float *q = (float *) c->trace_buf;
-    float *du = q; q += N; float *dv = q; q += N; float *did = q; q += N; float *dir = q; q += N; float *de2 = q; q += 2 * N; float *doth = q; q += N;
-    float *den = q; q += 2 * N; float *dms = q; q += N; float *dlh = q; q += N; float *djb = q; q += 10 * N;
-    float *dpart = q; q += grid * INIT_NACC; unsigned *dcnt = (unsigned *) q; q += 4;
-    q = (float *) (((uintptr_t) q + 7) & ~(uintptr_t) 7);
-    double *dout = (double *) q; q += 2 * INIT_NACC;
-    unsigned char *dg = (unsigned char *) q, *dgn = dg + N;
-#define IN_H2D(dst_, src_, bytes_) CUDA_CHECK_RET(c, cudaMemcpyAsync(dst_, src_, bytes_, cudaMemcpyHostToDevice, c->stream))
-    IN_H2D(du, u, 4 * N); IN_H2D(dv, v, 4 * N); IN_H2D(did, idepth_new, 4 * N); IN_H2D(dir, iR, 4 * N); IN_H2D(de2, energy2, 8 * N); IN_H2D(doth, outlierTH, 4 * N);
-    IN_H2D(dg, isGood, N);
-#undef IN_H2D
-    CUDA_CHECK_RET(c, cudaMemsetAsync(den, 0, 4 * (size_t) (2 + 1 + 1 + 10) * N, c->stream));      // energy_new, maxstep, lastHessian_new, Jb
-    CUDA_CHECK_RET(c, cudaMemsetAsync(dcnt, 0, 16, c->stream));
-    A.u = du; A.v = dv; A.idepth_new = did; A.iR = dir; A.energy2 = de2; A.outlierTH = doth; A.isGood = dg;
-    A.isGood_new = dgn; A.energy_new2 = den; A.maxstep = dms; A.lastHessian_new = dlh; A.Jb = djb;
-    A.partials = dpart; A.counter = dcnt; A.out = dout;
+    RET_IF(trace_carve(c, [&](Arena &R) { init_calc_res_regions(R, N, grid, A); }));
+    H2D(A.u, u, 4 * N); H2D(A.v, v, 4 * N); H2D(A.idepth_new, idepth_new, 4 * N); H2D(A.iR, iR, 4 * N); H2D(A.energy2, energy2, 8 * N);
+    H2D(A.outlierTH, outlierTH, 4 * N); H2D(A.isGood, isGood, N);
+    CUDA_CHECK_RET(c, cudaMemsetAsync(A.energy_new2, 0, 4 * (size_t) (2 + 1 + 1 + 10) * N, c->stream));      // energy_new, maxstep, lastHessian_new, Jb
+    CUDA_CHECK_RET(c, cudaMemsetAsync(A.counter, 0, 16, c->stream));
     launch_init_calc_res(A, c->stream);
     LAUNCH_CHECK(c);
     double sums[INIT_NACC];
-    D2H(isGood_new, dgn, N); D2H(energy_new2, den, 8 * N); D2H(maxstep, dms, 4 * N); D2H(lastHessian_new, dlh, 4 * N); D2H(JbBuffer_new10, djb, 40 * N);
-    D2H(sums, dout, sizeof(sums));
+    D2H(isGood_new, A.isGood_new, N); D2H(energy_new2, A.energy_new2, 8 * N); D2H(maxstep, A.maxstep, 4 * N); D2H(lastHessian_new, A.lastHessian_new, 4 * N);
+    D2H(JbBuffer_new10, A.Jb, 40 * N);
+    D2H(sums, A.out, sizeof(sums));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     // acc9.H / acc9SC.H -> H_out, b_out, H_out_sc, b_out_sc (:390-403)
     int k = 0;
@@ -2687,8 +2579,6 @@ extern "C" int ldso_b200_get_energy(ldso_b200_ctx *c, double *energy, int *canbr
     return LDSO_B200_OK;
 }
 
-#define D2H(dst, src, bytes) do { if (dst) CUDA_CHECK_RET(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream)); } while (0)
-
 // one D2H of the contiguous result range into the pinned mirror (valid until the next launch)
 // Optional hint: queue the read-back of everything the getters below return (solution, point and residual arrays) into
 // pinned staging memory right behind the work already on the stream, without blocking. The next getter then only waits
@@ -2879,34 +2769,20 @@ extern "C" int ldso_b200_posegraph_optimize(ldso_b200_ctx *c, int nV, double *q4
     for (int v = 0; v < nV; v++) ib[v + 1] += ib[v];
     { std::vector<int> pos(ib.begin(), ib.end() - 1); for (int e = 0; e < nE; e++) { inc[pos[ei[e]]++] = 2 * e; inc[pos[ej[e]]++] = 2 * e + 1; } }
     const int nbv = (nV + PG_WARPS - 1) / PG_WARPS, nbe = (nE + PG_WARPS - 1) / PG_WARPS;
-    // one device block
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t) 255; return o; };
-    const size_t o_q = take(32 * (size_t) nV), o_t = take(24 * (size_t) nV), o_ei = take(4 * (size_t) nE), o_ej = take(4 * (size_t) nE), o_mq = take(32 * (size_t) nE),
-                 o_mt = take(24 * (size_t) nE), o_info = take(392 * (size_t) nE), o_Hii = take(392 * (size_t) nE), o_Hij = take(392 * (size_t) nE), o_Hjj = take(392 * (size_t) nE),
-                 o_bi = take(56 * (size_t) nE), o_bj = take(56 * (size_t) nE), o_chi = take(8 * (size_t) nE), o_ib = take(4 * ((size_t) nV + 1)), o_inc = take(8 * (size_t) nE),
-                 o_D = take(392 * (size_t) nV), o_Di = take(392 * (size_t) nV), o_b = take(56 * (size_t) nV), o_x = take(56 * (size_t) nV), o_r = take(56 * (size_t) nV),
-                 o_z = take(56 * (size_t) nV), o_p0 = take(56 * (size_t) nV), o_p1 = take(56 * (size_t) nV), o_Ap = take(56 * (size_t) nV),
-                 o_part = take(8 * (size_t) std::max(nbv, nbe)), o_scal = take(64), o_cnt = take(16);
-    char *B = nullptr;
-    CUDA_CHECK_RET(c, cudaMalloc(&B, off));
-    struct Free { char *p; ~Free() { if (p) cudaFree(p); } } guard{B};
-    CUDA_CHECK_RET(c, cudaMemsetAsync(B, 0, off, c->stream));
-#define PG_UP(o, src, bytes) CUDA_CHECK_RET(c, cudaMemcpyAsync(B + (o), src, bytes, cudaMemcpyHostToDevice, c->stream))
-    PG_UP(o_q, q4, 32 * (size_t) nV); PG_UP(o_t, t3, 24 * (size_t) nV); PG_UP(o_ei, ei, 4 * (size_t) nE); PG_UP(o_ej, ej, 4 * (size_t) nE);
-    PG_UP(o_mq, mq4, 32 * (size_t) nE); PG_UP(o_mt, mt3, 24 * (size_t) nE); PG_UP(o_info, info49, 392 * (size_t) nE);
-    PG_UP(o_ib, ib.data(), 4 * ((size_t) nV + 1)); PG_UP(o_inc, inc.data(), 8 * (size_t) nE);
-#undef PG_UP
-    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));      // pageable sources
     PgGraph g;
+    Arena S;
+    posegraph_regions(S, nV, nE, g);
+    char *B = nullptr;
+    CUDA_CHECK_RET(c, cudaMalloc(&B, S.off));
+    struct Free { char *p; ~Free() { if (p) cudaFree(p); } } guard{B};
+    Arena D(B);
+    posegraph_regions(D, nV, nE, g);
+    CUDA_CHECK_RET(c, cudaMemsetAsync(B, 0, S.off, c->stream));
+    H2D(g.q, q4, 32 * (size_t) nV); H2D(g.t, t3, 24 * (size_t) nV); H2D(g.ei, ei, 4 * (size_t) nE); H2D(g.ej, ej, 4 * (size_t) nE);
+    H2D(g.mq, mq4, 32 * (size_t) nE); H2D(g.mt, mt3, 24 * (size_t) nE); H2D(g.info, info49, 392 * (size_t) nE);
+    H2D(g.inc_begin, ib.data(), 4 * ((size_t) nV + 1)); H2D(g.inc, inc.data(), 8 * (size_t) nE);
+    CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));      // pageable sources
     g.nV = nV; g.nE = nE; g.fixed = fixed;
-    g.q = (double *) (B + o_q); g.t = (double *) (B + o_t); g.ei = (const int *) (B + o_ei); g.ej = (const int *) (B + o_ej);
-    g.mq = (const double *) (B + o_mq); g.mt = (const double *) (B + o_mt); g.info = (const double *) (B + o_info);
-    g.Hii = (double *) (B + o_Hii); g.Hij = (double *) (B + o_Hij); g.Hjj = (double *) (B + o_Hjj); g.bi = (double *) (B + o_bi); g.bj = (double *) (B + o_bj);
-    g.chi2e = (double *) (B + o_chi); g.inc_begin = (const int *) (B + o_ib); g.inc = (const int *) (B + o_inc);
-    g.D = (double *) (B + o_D); g.Dinv = (double *) (B + o_Di); g.b = (double *) (B + o_b); g.x = (double *) (B + o_x); g.r = (double *) (B + o_r);
-    g.z = (double *) (B + o_z); g.p0 = (double *) (B + o_p0); g.p1 = (double *) (B + o_p1); g.Ap = (double *) (B + o_Ap);
-    g.part = (double *) (B + o_part); g.scal = (double *) (B + o_scal); g.counter = (unsigned *) (B + o_cnt);
     int total_cg = 0;
     const int chunk = 10;
     for (int it = 0; it <= iterations; it++) {
@@ -3088,19 +2964,18 @@ extern "C" int ldso_b200_tracker_track_batch(ldso_b200_ctx *c, int n, const doub
     A.huberTH = c->S.huberTH; A.coarseCutoffTH = c->S.coarseCutoffTH; A.affineOptModeA = c->S.affineOptModeA; A.affineOptModeB = c->S.affineOptModeB;
     A.coarsestLvl = coarsestLvl;
     for (int i = 0; i < 5; i++) A.minResForAbort[i] = NAN;
-    RET_IF(trace_reserve(c, (sizeof(TrkHypothesis) + sizeof(TrkTrackOut)) * (size_t) n + 64));
-    TrkHypothesis *dh = (TrkHypothesis *) c->trace_buf;
-    TrkTrackOut *dout = (TrkTrackOut *) (dh + n);
+    TrackBatchScratch s;
+    RET_IF(trace_carve(c, [&](Arena &R) { track_batch_regions(R, (size_t) n, s); }));
     std::vector<TrkHypothesis> hh(n);
     for (int i = 0; i < n; i++) {
         memcpy(hh[i].R, R9_each + 9 * i, 72); memcpy(hh[i].t, t3_each + 3 * i, 24);
         hh[i].aff_a = aff2_each[2 * i]; hh[i].aff_b = aff2_each[2 * i + 1];
     }
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(dh, hh.data(), sizeof(TrkHypothesis) * n, cudaMemcpyHostToDevice, c->stream));
-    k_trk_track<<<n, TRK_TRACK_THREADS, 0, c->stream>>>(A, dout, dh);
+    H2D(s.hyp, hh.data(), sizeof(TrkHypothesis) * n);
+    k_trk_track<<<n, TRK_TRACK_THREADS, 0, c->stream>>>(A, s.out, s.hyp);
     LAUNCH_CHECK(c);
     std::vector<TrkTrackOut> ho(n);
-    CUDA_CHECK_RET(c, cudaMemcpyAsync(ho.data(), dout, sizeof(TrkTrackOut) * n, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(c, cudaMemcpyAsync(ho.data(), s.out, sizeof(TrkTrackOut) * n, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(c, cudaStreamSynchronize(c->stream));
     for (int i = 0; i < n; i++) {
         if (R9_out) memcpy(R9_out + 9 * i, ho[i].R, 72);
